@@ -1,14 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- ViL-Small 224x224 bf16 training throughput (images/sec) on N B200s, with the
-Vision-Longformer attention hot path running on the vil_attn sm_100a kernels.
+"""bench.py -- ViL-Small 224x224 bf16 training throughput (images/sec) on N H100s, with the
+Vision-Longformer attention hot path running on the vil_attn sm_90a kernels.
 
-Contract (see the task statement):  python bench.py --gpus N --steps K --warmup W  prints ONE JSON line.
+python bench.py --gpus N --steps K --warmup W  prints ONE JSON line.
   value      : whole-job images/sec, inputs resident in HBM, CUDA-event timed, max over ranks
   e2e        : same step through the public module API with pinned-HOST images copied H2D and the loss
                read back D2H inside the timed region
   roofline   : the dominant hot-path kernel, timed alone with CUDA events inside this process
   cpu_baseline: the oracle port of the reference's CPU path (same model, small batch) on the host cores
   --impl reference : only the CPU arm (reference algorithm port), same metric / config
+  --dump-outputs DIR: after the timed steps, the loss, logits and a fixed sample of the parameter gradients of the last
+               timed step as DIR/<name>.npy (inputs and initial weights are seeded: equal arguments, equal inputs)
 """
 from __future__ import annotations
 
@@ -30,23 +32,19 @@ PER_GPU_BATCH = 256           # BASELINE config 3: synthetic ImageNet-shape batc
 MODEL, IMG = "vil_small", 224
 
 
-def ncu_traffic(key):
-    """DRAM bytes per launch measured by `ncu --set full` for this kernel (profiles/ncu_traffic.json, written by
-    tools/ncu_traffic.py from the committed capture); None when the capture does not cover it."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")
-    try:
-        with open(path) as f:
-            return json.load(f)[key]["dram_bytes"]
-    except (OSError, KeyError, ValueError):
-        return None
-
-
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        d = json.load(open(path))
-        return d["hbm_gbs"], d["bf16_tflops"], "measured (MEASURED_PEAKS.json, burst)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, 989.0, "H100 SXM data sheet (HBM3 3.35 TB/s, dense bf16 989 TFLOP/s at 700 W); not measured"
+
+
+def gpu_info(index=0):
+    """name and power limit of the card the numbers were measured on"""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader"], capture_output=True, text=True, timeout=10).stdout.strip()
+        name, power, clk = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit": power, "sm_max_clock": clk}
+    except Exception:
+        return {"name": torch.cuda.get_device_name(index), "power_limit": None, "sm_max_clock": None}
 
 
 # ------------------------------------------------------------------------------------------ clocks
@@ -125,9 +123,8 @@ def kernel_microbench(dev, reps=10, variants=True):
     """BASELINE config 2: attention-operator-only fwd / bwd at the ViL-Small hot-layer shapes, B=256, bf16, in the
     PRODUCTION layout (q / k / v = strided views of the query / kv Linear outputs, head-merged output, gradients written
     into Linear-layout buffers), timed with CUDA events on the launching stream; the tensors of one call (>= 0.6 GB per
-    shape) are cycled through 3 distinct buffer sets so consecutive reps cannot hit L2 (126 MB).
-    Per shape: the fused round-2 pipeline (default) and, for reference, the round-1 multi-kernel pipeline
-    (VIL_FLAG_UNFUSED); `variants` adds exact=1 and rpe-on timings of the fused/default path."""
+    shape) are cycled through 3 distinct buffer sets so consecutive reps cannot hit L2 (50 MB).
+    `variants` adds exact=1 and rpe-on timings."""
     from vision_longformer_b200 import _lib, vil_attention_raw_backward, vil_attention_raw_forward
     res = {}
     B = PER_GPU_BATCH
@@ -193,7 +190,6 @@ def kernel_microbench(dev, reps=10, variants=True):
         flops, byts = algorithmic_work(nx, ny, w, g, H, M)
         r = {"layout": "strided views of the query / kv Linear outputs (production)", "flops_fwd": flops * B, "bytes_fwd": byts * B}
         r.update(bench_one())
-        r["round1_pipeline"] = bench_one(flags=_lib.VIL_FLAG_UNFUSED)
         if variants:
             fl1, _ = algorithmic_work(nx, ny, w, g, H, M, exact=1)
             r["exact1"] = dict(bench_one(exact=1, passes=False), flops_fwd=fl1 * B)
@@ -209,7 +205,7 @@ def epilogue_microbench(dev, reps=10):
     """SURVEY.md section 8 (f) row 4 kernels (residual add + DropPath scale + deferred bias + LayerNorm; bias + GELU; column-sum bias
     gradient) at the ViL-Small token streams, B=256, through the C ABI on preallocated buffers (no autograd / allocator in the
     timed region): pure HBM kernels, so the figure of merit is algorithmic bytes / time against the measured HBM peak.
-    CUDA events on the launching stream, 3 buffer sets cycled (one call moves >= 0.2 GB: nothing survives in the 126 MB L2)."""
+    CUDA events on the launching stream, 3 buffer sets cycled (one call moves >= 0.2 GB: nothing survives in the 50 MB L2)."""
     from vision_longformer_b200 import _lib, epilogue as ep
     res = {}
     B = PER_GPU_BATCH
@@ -254,8 +250,7 @@ def epilogue_microbench(dev, reps=10):
             ("bias_gelu_bwd", lambda s: ep.bias_act_raw_backward(s["da"], s["z"], b1, s["dz"], db1, ws_g, _lib.VIL_ACT_GELU),
              4 * e * (2 + 2 + 2)),                                     # da, z -> dz (+ d_bias); 2 launches
             ("colsum", lambda s: ep.bias_act_raw_backward(s["da"], None, None, None, db1, ws_c, _lib.VIL_ACT_NONE), 4 * e * 2),
-            # context: what a plain device copy of the bias_gelu_fwd tensor achieves at THIS size (the 6571 GB/s peak was measured on
-            # a 2 x 2 GiB copy; these streams are 0.15 - 1.2 GB and pay launch / ramp-up / tail on 60 - 300 us kernels)
+            # context: what a plain device copy of the bias_gelu_fwd tensor achieves at THIS size
             ("torch_copy_same_size", lambda s: s["a"].copy_(s["z"]), 4 * e * (2 + 2)))
         r = {"rows": rows, "C": C}
         for name, fn, byts in kernels:
@@ -319,6 +314,25 @@ def config5_sweep(dev, B=8, img=512, reps=10):
     return out
 
 
+# ------------------------------------------------------------------------------------------ output dump
+def dump_outputs(out_dir, net, loss, logits, sample=4096):
+    """What the timed step hands its caller - the loss, the logits and the parameter gradients (a fixed sample of
+    `sample` entries per parameter, seeded, so two builds compare entry for entry) - as float32 / float64 .npy files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss.item()], dtype=np.float64))
+    np.save(os.path.join(out_dir, "logits.npy"), logits.detach().float().cpu().numpy())
+    gen = torch.Generator().manual_seed(0)
+    parts = []
+    for _, p in sorted(net.named_parameters(), key=lambda kv: kv[0]):
+        if p.grad is None:
+            continue
+        g = p.grad.detach().float().flatten()
+        idx = torch.randperm(g.numel(), generator=gen)[:sample].sort().values
+        parts.append(g[idx.to(g.device)].cpu())
+    np.save(os.path.join(out_dir, "grad_sample.npy"), torch.cat(parts).numpy())
+
+
 # ------------------------------------------------------------------------------------------ CPU arm
 def cpu_training_throughput(steps, warmup, batch=4):
     """The reference's CPU path, restated (oracle port, `chunked_attention` with the hand-written backward
@@ -326,8 +340,7 @@ def cpu_training_throughput(steps, warmup, batch=4):
     from oracle.vil_oracle import OracleLong2DSCSelfAttention
     from vision_longformer_b200 import build_vil
     torch.manual_seed(0)
-    # torch's CPU thread pool collapses on many-core hosts for this op mix (measured on the 128-core GPU box:
-    # 157 s/step with 128 threads vs ~2 s/step with 8): cap the pool and report the threads actually used.
+    # torch's CPU thread pool collapses on many-core hosts for this op mix: cap the pool and report the threads used.
     cores = min(os.cpu_count() or 1, 16)
     torch.set_num_threads(cores)
     net = build_vil(MODEL, img_size=IMG, attn_cls=OracleLong2DSCSelfAttention).train()
@@ -347,18 +360,6 @@ def cpu_training_throughput(steps, warmup, batch=4):
     return batch * len(times) / total, total / len(times) * 1e3, cores, batch
 
 
-def port_cost_note():
-    """The CPU arm is the oracle PORT of the reference algorithm (the reference tree does not exist on the GPU box).  Its
-    cost relative to the real reference MsViT on identical cores was measured in the authoring container
-    (tools/port_vs_reference.py -> profiles/r02_port_vs_reference.json) and is reported with the number."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "r02_port_vs_reference.json")))
-        return {"port_over_reference_time_ratio": d["port_over_reference_time_ratio"],
-                "ratio_source": "profiles/r02_port_vs_reference.json (reference MsViT vs oracle port, same cores, authoring container)"}
-    except (OSError, KeyError, ValueError):
-        return {}
-
-
 def run_reference_arm(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -371,7 +372,7 @@ def run_reference_arm(args):
             "config": {"workload": f"ViL-Small 224x224 training step (fwd+bwd+AdamW), batch {batch} (bounded CPU sample "
                                    f"of the {PER_GPU_BATCH}/GPU workload)", "attn": "oracle port of ATTN_TYPE=longformerhand"},
             "cpu_baseline": {"value": ips, "unit": "images/sec", "cores": cores, "kind": "port",
-                             "sample": f"{steps} timed steps of batch {batch}, fp32, torch CPU threads={cores}", **port_cost_note()},
+                             "sample": f"{steps} timed steps of batch {batch}, fp32, torch CPU threads={cores}"},
             "e2e": {"value": ips, "unit": "images/sec", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
 
@@ -391,6 +392,7 @@ def main():
     ap.add_argument("--no-microbench", action="store_true")
     ap.add_argument("--micro-only", action="store_true", help="only the attention-kernel microbench (BASELINE config 2)")
     ap.add_argument("--config5", action="store_true", help="BASELINE config 5: ViL-Base-Deep 512x512 backbone-forward window sweep")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)
@@ -445,11 +447,12 @@ def main():
 
     def step(x, y):
         with torch.autocast("cuda", dtype=torch.bfloat16):
-            loss = torch.nn.functional.cross_entropy(model(x), y)
+            logits = model(x)
+            loss = torch.nn.functional.cross_entropy(logits, y)
         opt.zero_grad(set_to_none=True)
         loss.backward()
         opt.step()
-        return loss
+        return loss, logits
 
     def sync_all():
         if world > 1:
@@ -474,12 +477,14 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            step(x_dev, y_dev)
+            last = step(x_dev, y_dev)
         e1.record()
         sync_all()
     launches = _lib.launch_count() - launches0
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     clocks = clk.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, net, *last)
 
     # ---- end-to-end timing: every step's images / labels are copied from PINNED HOST memory inside the timed region and
     # the loss is read back every step.  The copy of step i+1 runs on a side stream while step i computes (double-buffered
@@ -508,7 +513,7 @@ def main():
                 prefetch(i + 1)
             cur.wait_event(ready[i & 1])
             xb, yb = stage[i & 1]
-            loss = step(xb, yb)
+            loss, _ = step(xb, yb)
             freed[i & 1].record(cur)
             last = loss.item()                                # D2H read of the step's result
         return last
@@ -537,10 +542,10 @@ def main():
             "unit": "images/sec", "n_gpus": world, "steps": steps, "warmup": warmup, "ms_per_step": ms_total / steps,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": f"{arch} {img}x{img} bf16 training step (fwd+bwd+fused AdamW), {B} img/GPU, "
-                                   f"ATTN_TYPE=longformerhand -> vil_attn sm_100a kernels, w={wins} in the longformer stages, "
+                                   f"ATTN_TYPE=longformerhand -> vil_attn sm_90a kernels, w={wins} in the longformer stages, "
                                    f"SW_EXACT=0, rpe off (published arch string), DDP over NCCL when n_gpus>1",
                        "arch": arch, "img_size": img, "global_batch": world * B, "parallelism": f"dp{world}",
-                       "l2": "per-step activation working set is several GB (>> 126 MB L2); no explicit flush",
+                       "l2": "per-step activation working set is several GB (>> 50 MB L2); no explicit flush",
                        "harness": "reference block structure; residual add + DropPath + deferred bias + LayerNorm and bias + GELU in the "
                                   "vil_addnorm / vil_bias_act kernels (fused_residual=True), NHWC patch-merge convolutions; GEMMs cuBLAS, dense "
                                   "s0-stage attention cuDNN SDPA"},
@@ -548,7 +553,7 @@ def main():
                     "h2d_bytes_per_step": x_host.numel() * 4 + y_host.numel() * 8, "d2h_bytes_per_step": 4,
                     "ms_per_step": ms_e2e / steps, "last_loss": loss_value,
                     "h2d": "pinned host -> device every step on a side stream, overlapped with the previous step"},
-            "gpu_launches": launches, "clocks": clocks, "attn_family": _lib.last_impl()}
+            "gpu_launches": launches, "clocks": clocks, "gpu": gpu_info(local), "attn_family": _lib.last_impl()}
 
     if world == 1 and not args.no_microbench:
         mb = kernel_microbench(dev)
@@ -567,19 +572,14 @@ def main():
         achieved = kbytes / (ms * 1e-3) / 1e9
         line["roofline"] = {"bound": "hbm", "kernel": f"{name}[{tag}] ({r['family_fwd'] if name == 'fwd' else r['family_bwd']})",
                             "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
-                            "traffic": ncu_traffic(f"{name}[{tag}]"),
-                            "traffic_source": "profiles/ncu_traffic.json (ncu --set full capture of this build, committed)",
                             "algorithmic_bytes": kbytes, "peak_source": peak_src, "kernel_ms": ms,
                             "tensor_frac": kflops / (ms * 1e-3) / 1e12 / tflops}
         # whole operator (SURVEY.md section 8(d) accounting: backward = 2 x forward bytes / flops), 1 x S1 + 2 x S2 layers
         op_ms = sum(r2["fwd_ms"] + r2["bwd_ms"] for r2 in mb.values()) + mb["S2"]["fwd_ms"] + mb["S2"]["bwd_ms"]
         op_bytes = 3 * (mb["S1"]["bytes_fwd"] + 2 * mb["S2"]["bytes_fwd"])
         op_flops = 3 * (mb["S1"]["flops_fwd"] + 2 * mb["S2"]["flops_fwd"])
-        old_ms = sum(r2["round1_pipeline"]["fwd_ms"] + r2["round1_pipeline"]["bwd_ms"] for r2 in mb.values()) + \
-            mb["S2"]["round1_pipeline"]["fwd_ms"] + mb["S2"]["round1_pipeline"]["bwd_ms"]
         line["roofline"]["operator"] = {"ms_fwd_bwd_3_layers": op_ms, "hbm_frac": op_bytes / (op_ms * 1e-3) / 1e9 / hbm,
-                                        "tensor_frac": op_flops / (op_ms * 1e-3) / 1e12 / tflops,
-                                        "round1_pipeline_ms": old_ms}
+                                        "tensor_frac": op_flops / (op_ms * 1e-3) / 1e12 / tflops}
         line["kernel_bench"] = mb
         line["kernel_bench"]["hot_path_ms_per_256img"] = op_ms      # 1x S1 + 2x S2 layers, fwd+bwd
         line["kernel_bench"]["hot_path_images_per_sec"] = PER_GPU_BATCH / (op_ms * 1e-3)
@@ -589,8 +589,7 @@ def main():
         ips, ms, cores, batch = cpu_training_throughput(steps=2, warmup=1)
         line["cpu_baseline"] = {"value": ips, "unit": "images/sec", "cores": cores, "kind": "port",
                                 "sample": f"2 timed ViL-Small training steps of batch {batch}, fp32 CPU, oracle port of "
-                                          f"the reference's sliding-chunk algorithm ({ms:.0f} ms/step)",
-                                **port_cost_note()}
+                                          f"the reference's sliding-chunk algorithm ({ms:.0f} ms/step)"}
     print(json.dumps(line))
     if world > 1:
         torch.distributed.barrier()

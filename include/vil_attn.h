@@ -1,6 +1,6 @@
 /*
- * vil_attn.h -- C ABI of the B200 (sm_100a) Vision-Longformer attention library
- *               (libvil_attn_sm100.so).
+ * vil_attn.h -- C ABI of the H100 (sm_90a) Vision-Longformer attention library
+ *               (libvil_attn.so).  Entry-point names keep the _sm100 suffix of their first target.
  *
  * This is the drop-in boundary for ONE hot path of microsoft/vision-longformer:
  * the "2-D sliding-chunk local + global-token" attention that
@@ -54,9 +54,9 @@ enum { VIL_F32 = 0, VIL_BF16 = 1, VIL_F16 = 2 };
 
 /* kernel family selection */
 enum {
-  VIL_IMPL_AUTO    = 0, /* tcgen05 path when the configuration is covered, else SIMT */
+  VIL_IMPL_AUTO    = 0, /* wgmma path when the configuration is covered, else SIMT */
   VIL_IMPL_SIMT    = 1, /* CUDA-core fp32 path: every (w, exact, mode, nglo, D<=128) incl. fp32 I/O */
-  VIL_IMPL_TCGEN05 = 2  /* TMA + tcgen05/TMEM path (bf16/fp16): error if the configuration is not covered */
+  VIL_IMPL_WGMMA   = 2  /* wgmma tensor-core path (bf16/fp16, D <= 64): error if the configuration is not covered */
 };
 
 /* VilAttnParams.flags */
@@ -64,10 +64,9 @@ enum {
   /* PARITY BUILD (tests only, SURVEY.md section 8(c) protocol step 1): q/k/v/d_o stay bf16/fp16 but every OUTPUT tensor
      (o, og, dq, dk, dv, dqg, dkg, dvg) is fp32 - VilTensor4 strides then count fp32 elements.  It isolates the
      kernels' internal error (bf16 P / dS operands, fp32 accumulation) from the rounding of the stored result.
-     tcgen05 family only. */
+     wgmma family only. */
   VIL_FLAG_F32_OUT = 1,
-  /* run the round-1 multi-kernel pipeline (separate global-token / delta / re-ordering kernels) even where the fused
-     kernels apply: kept for A/B timing and as the cross-check of the fused path in the tests */
+  /* accepted for ABI compatibility: every family runs one pipeline, so it changes nothing */
   VIL_FLAG_UNFUSED = 2
 };
 
@@ -136,17 +135,17 @@ int         vil_attn_abi_version(void);
 const char* vil_attn_last_error(void);
 /* number of kernel launches this library has issued since it was loaded (all threads) */
 int64_t     vil_attn_launch_count(void);
-/* name of the kernel family the last successful fwd / bwd call on this thread used ("simt" / "tcgen05") */
+/* name of the kernel family the last successful fwd / bwd call on this thread used ("simt" / "wgmma") */
 const char* vil_attn_last_impl(void);
-/* name of the main kernel variant the last tcgen05 forward / backward launch on this thread used ("fwd4", "fwd3", ...;
+/* name of the main kernel the last wgmma forward / backward launch on this thread used ("wgmma_fwd", "wgmma_bwd";
    "" when the family does not report one) - lets tests assert which variant ran */
 const char* vil_attn_last_kernel(void);
 
 /* scratch size needed by the forward (backward == 0) or backward (backward != 0) call; < 0 on error */
 int64_t vil_attn_workspace_bytes(const VilAttnParams* p, int backward);
 
-/* returns 1 if the tcgen05 family covers this configuration, 0 if only the SIMT family does, < 0 on error */
-int vil_attn_tcgen05_supported(const VilAttnParams* p);
+/* returns 1 if the wgmma family covers this configuration, 0 if only the SIMT family does, < 0 on error */
+int vil_attn_wgmma_supported(const VilAttnParams* p);
 
 /* fused forward: o, og, lse, lse_g.  `stream` is a cudaStream_t. */
 int vil_attn_fwd_sm100(const VilAttnParams* p, void* stream);

@@ -1,7 +1,7 @@
-"""Generate golden vectors by IMPORTING THE UNMODIFIED REFERENCE (/root/reference).
+"""Generate golden vectors by IMPORTING THE UNMODIFIED REFERENCE.
 
-Run in the authoring container only (the reference does not travel to the GPU
-box):   python oracle/make_golden.py
+Run where a checkout of the reference exists (the tests themselves never need it):
+    VIL_REFERENCE_SRC=<reference checkout>/src python oracle/make_golden.py
 Outputs small fixtures under tests/golden/*.pt which ARE committed.
 
 What is pinned
@@ -18,6 +18,12 @@ What is pinned
   pinning the stock-PyTorch harness in vision_longformer_b200/msvit.py.
 * `mask_*.pt`  : raw outputs of the three reference mask builders
   (slidingchunk_2d.py:249-318) for the oracle's closed forms.
+* `oracle_fresh_seed.pt` : one more module configuration (w=3, nglo=2, separate
+  global weights) with its own seed, beyond the `attn_*` cases.
+* `dropin_reference.pt` : what the drop-in class must reproduce of the reference's own
+  `MsViT` / `Long2DSCSelfAttention` (tests/test_dropin_reference.py): state_dict
+  keys and shapes, parameter count, public attributes and `compute_macs` of the
+  attention modules, `relative_position_index`.
 """
 import os
 import random
@@ -26,7 +32,7 @@ import types
 
 import torch
 
-REF = "/root/reference/src"
+REF = os.environ.get("VIL_REFERENCE_SRC", "")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 
@@ -172,9 +178,47 @@ def gen_masks(sc):
     print("wrote masks.pt", len(out))
 
 
+DROPIN_TINY = "l1,h1,d48,n1,s1,g1,p4,f7_l2,h3,d96,n1,s1,g1,p2,f7_l3,h3,d192,n2,s0,g1,p2,f7_l4,h6,d384,n1,s0,g0,p2,f7"
+DROPIN_ATTRS = ("Nglo", "num_heads", "head_dim", "attention_window", "only_glo", "scale", "exact", "rpe")
+DROPIN_RPE_KW = dict(dim=48, num_heads=3, qkv_bias=True, w=4, nglo=2, sharew=False, rpe=True, exact=1, mode=0)
+
+
+def gen_dropin(Cls, MsViT):
+    torch.manual_seed(0)
+    net = MsViT(arch=DROPIN_TINY, img_size=224, num_classes=10, drop_path_rate=0.1, norm_embed=True, sharew=True,
+                attn_type="longformerhand", sw_exact=0, mode=1, ln_eps=1e-6)
+    attn = [m for m in net.modules() if isinstance(m, Cls)]
+    macs = []
+    for a in attn:
+        a.__flops__ = 0
+        type(a).compute_macs(a, (torch.zeros(1, a.Nglo + 56 * 56, a.num_heads * a.head_dim),), None)
+        macs.append(int(a.__flops__))
+    ref = Cls(autograd=False, **DROPIN_RPE_KW)
+    out = dict(arch=DROPIN_TINY, shapes={k: tuple(v.shape) for k, v in net.state_dict().items()},
+               n_params=sum(p.numel() for p in net.parameters()),
+               attrs=[{n: getattr(a, n) for n in DROPIN_ATTRS} for a in attn], macs_56x56=macs,
+               rpe_kwargs=DROPIN_RPE_KW, rpe_keys=sorted(ref.state_dict().keys()),
+               relative_position_index=ref.relative_position_index.clone())
+    torch.save(out, os.path.join(OUT, "dropin_reference.pt"))
+    print("wrote dropin_reference.pt", len(out["shapes"]), macs)
+
+
+def gen_fresh(Cls):
+    torch.manual_seed(1234)
+    kw = dict(dim=24, num_heads=2, w=3, nglo=2, exact=0, rpe=True, sharew=False, qkv_bias=True)
+    ref = Cls(autograd=False, **kw).double().eval()
+    x = torch.randn(2, 2 + 8 * 10, 24, dtype=torch.float64)
+    out = dict(kwargs=kw, state_dict={k: v.detach().clone() for k, v in ref.state_dict().items()}, x=x, nx=8, ny=10,
+               y=ref(x, 8, 10).detach())
+    torch.save(out, os.path.join(OUT, "oracle_fresh_seed.pt"))
+    print("wrote oracle_fresh_seed.pt")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     Cls, sc, MsViT = import_reference()
+    gen_fresh(Cls)
+    gen_dropin(Cls, MsViT)
     gen_masks(sc)
     for name, (B, nx, ny, kw, pick) in ATTN_CASES.items():
         gen_attn(name, B, nx, ny, kw, pick, Cls)

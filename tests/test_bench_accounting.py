@@ -1,6 +1,5 @@
 """bench.py's roofline accounting is pinned to the algorithmic work SURVEY.md section 8(d) computed for the BASELINE
 configs (per image, per layer, forward) - the `roofline.achieved` figure is built from these numbers."""
-import json
 import os
 import sys
 
@@ -33,31 +32,3 @@ def test_bytes_match_survey():
     _, b2 = bench.algorithmic_work(28, 28, 7, 1, 3, 64)
     assert b1 / 1e6 == pytest.approx(2.41, rel=2e-2)
     assert b2 / 1e6 == pytest.approx(1.21, rel=2e-2)
-
-
-def test_committed_ncu_traffic_is_close_to_the_algorithmic_bytes():
-    """DRAM traffic measured by ncu (profiles/ncu_traffic.json) must stay within 30 % of the algorithmic bytes of the
-    launch: a larger gap would mean wasted re-reads (the first thing the roofline section is there to catch)."""
-    with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-        tr = json.load(f)
-    # pass 1 reads q, k, v, dO and O and writes dq (6 tensors: O is read here since round 2); pass 2 reads q, k, v, dO, writes dk, dv
-    factor = {"fwd": 1.0, "fwd_local": 1.0, "bwd_dq": 6 / 4, "bwd_dkv": 6 / 4}
-    shapes = {"S1": (56, 56, 7, 1, 3, 32), "S2": (28, 28, 7, 1, 3, 64)}
-    # epilogue kernels (tools/epilogue_only.py streams, bf16 branch): bytes per (row, channel of the C-wide stream)
-    epi = {"addnorm_fwd": 4 + 2 + 4 + 2, "addnorm_bwd": 2 + 4 + 4 + 4 + 2, "bias_gelu_fwd": 4 * (2 + 2), "bias_gelu_bwd": 4 * (2 + 2 + 2),
-           "colsum": 2 * 2}
-    streams = {"S1": (256 * (1 + 56 * 56), 96), "S2": (256 * (1 + 28 * 28), 192)}
-    for key, rec in tr.items():
-        name, tag = key[:-4], key[-3:-1]
-        assert bench.ncu_traffic(key) == rec["dram_bytes"]
-        if name in epi:                                  # pure streaming kernels: nothing is read twice
-            rows, C = streams[tag]
-            algo = rows * C * epi[name]
-            assert 0.90 * algo < rec["dram_bytes"] < 1.10 * algo, (key, rec["dram_bytes"], algo)
-            continue
-        _, b = bench.algorithmic_work(*shapes[tag])
-        if name.endswith("merge"):                       # per-unit partials of the global rows: a few MB per launch
-            assert rec["dram_bytes"] < 0.03 * 256 * b, (key, rec["dram_bytes"])
-            continue
-        algo = 256 * b * factor[name]
-        assert 0.75 * algo < rec["dram_bytes"] < 1.30 * algo, (key, rec["dram_bytes"], algo)

@@ -66,7 +66,7 @@ def test_column_sum_plan_covers_every_row_and_column():
                 ncs = (G + 255) // 256
                 gs = (G + ncs - 1) // ncs
                 rpi = 256 // gs
-                want = (148 * 8) // ncs
+                want = (132 * 8) // ncs
                 per = max((rows + want - 1) // want, 4 * rpi)
                 nrs = max((rows + per - 1) // per, 1)
                 assert gs <= 256 and rpi >= 1 and ncs * gs >= G                        # every column group has a thread

@@ -1,4 +1,4 @@
-"""vision_longformer_b200: a B200-native (sm_100a) drop-in for ONE hot path of
+"""vision_longformer_b200: an H100-native (sm_90a) drop-in for ONE hot path of
 microsoft/vision-longformer - the 2-D sliding-chunk local + global-token attention that
 MODEL.VIT.MSVIT.ATTN_TYPE='longformerhand' selects.  See DESIGN.md / INTEGRATION.md."""
 from .attention import B200Long2DSCSelfAttention, make_dropin_class, relative_position_index

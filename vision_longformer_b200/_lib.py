@@ -1,8 +1,8 @@
-"""ctypes binding of libvil_attn_sm100.so (C ABI declared in include/vil_attn.h).
+"""ctypes binding of libvil_attn.so (C ABI declared in include/vil_attn.h).
 
 There is deliberately NO fallback: if the library is missing the import-time
 loader raises, and every op raises if CUDA is unavailable.  The library is
-built in-tree by `__graft_entry__.build()` (nvcc, sm_100a).
+built in-tree by `__graft_entry__.build()` (nvcc, sm_90a).
 """
 from __future__ import annotations
 
@@ -11,11 +11,11 @@ import os
 import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_NAME = "libvil_attn_sm100.so"
+LIB_NAME = "libvil_attn.so"
 LIB_PATH = os.environ.get("VIL_ATTN_LIB") or os.path.join(_HERE, LIB_NAME)   # override: debug builds only
 
 VIL_F32, VIL_BF16, VIL_F16 = 0, 1, 2
-VIL_IMPL_AUTO, VIL_IMPL_SIMT, VIL_IMPL_TCGEN05 = 0, 1, 2
+VIL_IMPL_AUTO, VIL_IMPL_SIMT, VIL_IMPL_WGMMA = 0, 1, 2
 VIL_E_BADARG, VIL_E_UNSUPPORTED, VIL_E_CUDA, VIL_E_WORKSPACE = -1, -2, -3, -4
 ABI_VERSION = 2
 VIL_FLAG_F32_OUT, VIL_FLAG_UNFUSED = 1, 2
@@ -23,7 +23,7 @@ VIL_FLAG_F32_OUT, VIL_FLAG_UNFUSED = 1, 2
 # every symbol include/vil_attn.h declares
 EXPORTS = (
     "vil_attn_abi_version", "vil_attn_last_error", "vil_attn_launch_count", "vil_attn_last_impl", "vil_attn_last_kernel",
-    "vil_attn_workspace_bytes", "vil_attn_tcgen05_supported", "vil_attn_fwd_sm100", "vil_attn_bwd_sm100",
+    "vil_attn_workspace_bytes", "vil_attn_wgmma_supported", "vil_attn_fwd_sm100", "vil_attn_bwd_sm100",
     "vil_layernorm_workspace_bytes", "vil_layernorm_fwd_sm100", "vil_layernorm_bwd_sm100",
     "vil_addnorm_workspace_bytes", "vil_addnorm_fwd_sm100", "vil_addnorm_bwd_sm100",
     "vil_bias_act_workspace_bytes", "vil_bias_act_fwd_sm100", "vil_bias_act_bwd_sm100",
@@ -102,7 +102,7 @@ def load() -> ctypes.CDLL:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc -gencode arch=compute_100a,code=sm_100a).  There is no CPU / PyTorch fallback.")
+                "(nvcc -gencode arch=compute_90a,code=sm_90a).  There is no CPU / PyTorch fallback.")
         lib = ctypes.CDLL(LIB_PATH)
         lib.vil_attn_abi_version.restype = ctypes.c_int
         lib.vil_attn_last_error.restype = ctypes.c_char_p
@@ -111,8 +111,8 @@ def load() -> ctypes.CDLL:
         lib.vil_attn_launch_count.restype = ctypes.c_int64
         lib.vil_attn_workspace_bytes.restype = ctypes.c_int64
         lib.vil_attn_workspace_bytes.argtypes = [ctypes.POINTER(VilAttnParams), ctypes.c_int]
-        lib.vil_attn_tcgen05_supported.restype = ctypes.c_int
-        lib.vil_attn_tcgen05_supported.argtypes = [ctypes.POINTER(VilAttnParams)]
+        lib.vil_attn_wgmma_supported.restype = ctypes.c_int
+        lib.vil_attn_wgmma_supported.argtypes = [ctypes.POINTER(VilAttnParams)]
         for fn in (lib.vil_attn_fwd_sm100, lib.vil_attn_bwd_sm100):
             fn.restype = ctypes.c_int
             fn.argtypes = [ctypes.POINTER(VilAttnParams), ctypes.c_void_p]

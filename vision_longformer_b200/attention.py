@@ -75,7 +75,7 @@ class B200Long2DSCSelfAttention(nn.Module):
             raise ValueError("longsc exact should be in [0,1,-1]!")
         self.exact = exact
         self.autograd = autograd        # accepted for signature parity; the fused op has one hand-written backward
-        self.impl = "auto"              # "auto" | "simt" | "tcgen05" (kernel family; see include/vil_attn.h)
+        self.impl = "auto"              # "auto" | "simt" | "wgmma" (kernel family; see include/vil_attn.h)
 
         self.rpe = rpe
         if rpe:
@@ -119,7 +119,7 @@ class B200Long2DSCSelfAttention(nn.Module):
         g, H = self.Nglo, self.num_heads
         assert g + Nloc == N, "Global dimension does not match!"
         if not x.is_cuda:
-            raise RuntimeError("B200Long2DSCSelfAttention only runs on a CUDA (sm_100a) device; there is no CPU "
+            raise RuntimeError("B200Long2DSCSelfAttention only runs on a CUDA (sm_90a) device; there is no CPU "
                                "fallback (use the reference module / oracle for CPU parity checks)")
         if self.attn_drop.p > 0 and self.training:
             raise NotImplementedError("attention dropout > 0 is not supported by the fused kernel "

@@ -1,4 +1,4 @@
-// C-ABI entry points of libvil_attn_sm100.so (see include/vil_attn.h).
+// C-ABI entry points of libvil_attn.so (see include/vil_attn.h).
 // Host-side only: argument validation (mirroring the reference's asserts / ValueErrors,
 // longformer2d.py:22,45-46,111 and slidingchunk_2d.py:331-343), geometry set-up, kernel
 // family selection and launches on the caller's stream.  No allocation, no host sync.
@@ -131,11 +131,11 @@ int run(const VilAttnParams* p, void* stream, bool bwd) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int tc_ok = vil::tc_supported(p, g, bwd);
   int impl = p->impl;
-  if (impl == VIL_IMPL_AUTO) impl = tc_ok ? VIL_IMPL_TCGEN05 : VIL_IMPL_SIMT;
-  if (impl == VIL_IMPL_TCGEN05) {
-    if (!tc_ok) return fail(VIL_E_UNSUPPORTED, "tcgen05 family does not cover this configuration: %s", vil::tc_why_not(p, g, bwd));
+  if (impl == VIL_IMPL_AUTO) impl = tc_ok ? VIL_IMPL_WGMMA : VIL_IMPL_SIMT;
+  if (impl == VIL_IMPL_WGMMA) {
+    if (!tc_ok) return fail(VIL_E_UNSUPPORTED, "the wgmma family does not cover this configuration: %s", vil::tc_why_not(p, g, bwd));
     rc = bwd ? vil::tc_backward(p, g, s) : vil::tc_forward(p, g, s);
-    if (rc == VIL_OK) g_last_impl = "tcgen05";
+    if (rc == VIL_OK) g_last_impl = "wgmma";
     return rc;
   }
   if (impl != VIL_IMPL_SIMT) return fail(VIL_E_BADARG, "impl must be VIL_IMPL_AUTO, _SIMT or _TCGEN05");
@@ -147,7 +147,7 @@ int run(const VilAttnParams* p, void* stream, bool bwd) {
 }  // namespace
 
 namespace vil {
-// hooks used by the tcgen05 family (vil_tc.cuh) for the kernels it shares with the SIMT family
+// hooks used by the wgmma family (vil_wgmma.cu) for the kernels it shares with the SIMT family
 int shared_fail(int code, const char* msg) { return fail(code, "%s", msg); }
 void count_launch() { VIL_LAUNCHED(); }
 void note_kernel(const char* name) { g_last_kernel = name; }
@@ -155,15 +155,16 @@ void note_kernel(const char* name) { g_last_kernel = name; }
 
 namespace {
 
+constexpr int kSMs = 132;                       // H100 SXM
+
 // backward grid: enough warps to cover HBM latency (up to 8 CTAs x 8 warps per SM), fewer for short streams so the
 // per-warp partial d_gamma / d_beta rows stay small next to the activations
 inline int ln_bwd_grid(long long rows) {
   long long g = rows / (vil::ln::kWarpsPerCta * 16);
-  if (g < 148) g = 148;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g < kSMs) g = kSMs;
+  if (g > kSMs * 8) g = kSMs * 8;
   return (int)g;
 }
-constexpr int kLnBwdGridMax = 148 * 8;
 
 int ln_check(const VilLayerNormParams* p, bool bwd) {
   if (p == nullptr) return fail(VIL_E_BADARG, "params is NULL");
@@ -190,7 +191,7 @@ int ln_launch(const VilLayerNormParams* p, cudaStream_t s, bool bwd) {
   if (p->rows == 0) return VIL_OK;
   if (!bwd) {
     long long ctas = (p->rows + vil::ln::kWarpsPerCta - 1) / vil::ln::kWarpsPerCta;
-    if (ctas > 148 * 8) ctas = 148 * 8;
+    if (ctas > kSMs * 8) ctas = kSMs * 8;
     vil::ln::layernorm_fwd<TX, TY, NPL><<<(unsigned)ctas, vil::ln::kWarpsPerCta * 32, 0, s>>>(
         static_cast<const TX*>(p->x), p->gamma, p->beta, static_cast<TY*>(p->y), p->mean, p->rstd, p->rows, p->C, p->eps);
     VIL_LAUNCHED();
@@ -262,12 +263,11 @@ int64_t vil_attn_workspace_bytes(const VilAttnParams* p, int backward) {
   int rc = make_geo(p, &g);
   if (rc) return rc;
   long long bytes = 256;
-  if (backward) bytes += vil::ws_off_tc(g) * 4;
-  bytes += vil::tc_workspace_bytes(p, g, backward != 0);
+  if (backward) bytes += vil::ws_floats(g) * 4;
   return bytes;
 }
 
-int vil_attn_tcgen05_supported(const VilAttnParams* p) {
+int vil_attn_wgmma_supported(const VilAttnParams* p) {
   vil::Geo g;
   int rc = make_geo(p, &g);
   if (rc) return rc;

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the vil_attn kernels (sm_100a).
+// Shared device/host helpers for the vil_attn kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -24,14 +24,9 @@ struct Geo {
   float scale;
 };
 
-// workspace layout (floats): [delta (B*H*Nloc)] [delta_g (B*H*g)] [tcgen05: lse2c, deltac (B*H*mx*my*64 each)] [lse2g, deltag]
+// backward workspace layout (floats): [delta (B*H*Nloc)] [delta_g (B*H*g)]
 inline long long ws_off_delta_g(const Geo& g) { return ((long long)g.B * g.H * g.Nloc + 63) & ~63LL; }
-inline long long ws_off_tc(const Geo& g) { return ws_off_delta_g(g) + (((long long)g.B * g.H * g.g + 63) & ~63LL); }
-inline int tc_pieces(int w) { if (w <= 8) return 1; const int pr = 64 / w; return (w + pr - 1) / pr; }
-inline long long ws_tc_floats(const Geo& g) { return 2LL * g.B * g.H * g.mx * g.my * tc_pieces(g.w) * 64; }
-// tcgen05 pass 2 with the global query rows folded in: lse2g, deltag (B*H*16 floats each) behind lse2c / deltac
-inline long long ws_off_tcg(const Geo& g) { return ws_off_tc(g) + ws_tc_floats(g); }
-inline long long ws_tcg_floats(const Geo& g) { return 2LL * g.B * g.H * 16; }
+inline long long ws_floats(const Geo& g) { return ws_off_delta_g(g) + (((long long)g.B * g.H * g.g + 63) & ~63LL); }
 
 struct T4 {             // device view (B,H,T,D), unit stride on D
   char* p;

@@ -1,5 +1,5 @@
 // TU: C-ABI entry points of the residual / LayerNorm / bias epilogue kernels (vil_epilogue.cuh; include/vil_attn.h).
-// Host side only: validation, grid sizing (multiples of the 148 SMs), launches on the caller's stream.  No allocation.
+// Host side only: validation, grid sizing (multiples of the 132 SMs of an H100 SXM), launches on the caller's stream.  No allocation.
 #include <cstdio>
 #include <cstdlib>
 #include "vil_host.cuh"
@@ -9,7 +9,7 @@ namespace {
 
 using namespace vil;
 
-constexpr int kSMs = 148;
+constexpr int kSMs = 132;
 
 int efail(int code, const char* msg) { return shared_fail(code, msg); }
 

@@ -1,4 +1,4 @@
-// Host-side glue shared by the translation units of libvil_attn_sm100.so.  The library is compiled as several TUs
+// Host-side glue shared by the translation units of libvil_attn.so.  The library is compiled as several TUs
 // (one per kernel family / pass, built in parallel by __graft_entry__.build()); every kernel lives entirely in one
 // TU, so no relocatable device code is needed.
 #pragma once
@@ -32,38 +32,10 @@ int simt_delta(const VilAttnParams* p, const Geo& g, cudaStream_t s);           
 // global key columns + global query rows; rmw_rows: keys whose dk / dv rows simt_bwd_grow still updates
 int simt_global_bwd(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_rows);
 
-// ---- vil_tc_dispatch.cu: the tcgen05 / TMA family
+// ---- vil_wgmma.cu: the tensor-core (wgmma) family
 const char* tc_why_not(const VilAttnParams* p, const Geo& g, bool bwd);
 int tc_supported(const VilAttnParams* p, const Geo& g, bool bwd);
-long long tc_workspace_bytes(const VilAttnParams* p, const Geo& g, bool bwd);
 int tc_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s);
 int tc_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-
-namespace tc {
-// per-kernel TUs (w <= 8: vil_tc_fwd.cu / vil_tc_dq.cu / vil_tc_dkv.cu; w in {12,15,31}: vil_tc_big_*.cu)
-int launch_fwd_local(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd_prep(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd_dq(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd_dkv(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-// fused forward (local + global query rows in one kernel + a tiny merge), vil_tc_fwd2.cu
-int launch_fwd2(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_fwd3(const VilAttnParams* p, const Geo& g, cudaStream_t s);      // 4-CTA/SM variant (vil_tc_fwd3.cu)
-int launch_fwd5(const VilAttnParams* p, const Geo& g, cudaStream_t s);      // key-row-block variant (vil_tc_fwd5.cu): w = 7, D <= 32
-bool fwd5_applies(const VilAttnParams* p, const Geo& g);
-bool fwd2_fuses_global_rows(const VilAttnParams* p, const Geo& g);
-long long fwd2_workspace_floats(const VilAttnParams* p, const Geo& g);
-// fused backward (vil_tc_bwd2.cu): pass 1 (+ delta, re-ordering, dq of the global rows), pass 2 (+ dk/dv of the global
-// key rows), merge of the per-unit partials
-bool bwd2_applies(const VilAttnParams* p, const Geo& g);
-bool bwd2_fuses_spare_rows(const VilAttnParams* p, const Geo& g);
-long long bwd2_workspace_floats(const VilAttnParams* p, const Geo& g);
-int launch_bwd2_dq(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd2_dkv(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd2_merge(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_fwd_local_big(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd_prep_big(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd_dq_big(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-int launch_bwd_dkv_big(const VilAttnParams* p, const Geo& g, cudaStream_t s);
-}  // namespace tc
 
 }  // namespace vil

@@ -144,7 +144,7 @@ int simt_dispatch(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd
 
 int simt_run(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
   if (out_f32(p) && p->dtype != VIL_F32)
-    return shared_fail(VIL_E_UNSUPPORTED, "VIL_FLAG_F32_OUT (parity build) is implemented by the tcgen05 family only");
+    return shared_fail(VIL_E_UNSUPPORTED, "VIL_FLAG_F32_OUT (parity build) is implemented by the wgmma family only");
   switch (p->dtype) {
     case VIL_F32:  return simt_dispatch<float>(p, g, s, bwd);
     case VIL_BF16: return simt_dispatch<__nv_bfloat16>(p, g, s, bwd);

@@ -3,7 +3,7 @@
 // Covers EVERY configuration of the reference operator (any w, exact in {0,1,-1},
 // mode in {-1,0,1..8}, any nglo, D <= 128 forward / D <= 64 backward, fp32 / bf16 /
 // fp16 I/O).  It is (a) the fp32 parity build (1e-5 vs the fp64 oracle), (b) the
-// path for configurations the tcgen05 family does not cover, and (c) the home of
+// path for configurations the wgmma family does not cover, and (c) the home of
 // the small global-token kernels that both families share.
 //
 // Math restated from the reference (closed forms verified in oracle/vil_oracle.py):
@@ -609,8 +609,7 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
               const float* __restrict__ lse_g, const float* __restrict__ delta_g,
               const float* __restrict__ g2l, const float* __restrict__ g2g,
               float* __restrict__ d_g2l, float* __restrict__ d_g2g, int accumulate, int rmw_rows) {
-  // rmw_rows: keys [0, rmw_rows) get their dkg / dvg rows updated here (all N, or only the g global keys when the
-  // tcgen05 pass 2 has already folded the global query rows into dk / dv of the local keys)
+  // rmw_rows: keys [0, rmw_rows) get their dkg / dvg rows updated here
   constexpr int LPR = HD / 8, RPW = 32 / LPR, ROWS = 8 * RPW;
   __shared__ float red[8];
   __shared__ float accs[8][HD];

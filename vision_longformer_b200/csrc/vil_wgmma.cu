@@ -1,0 +1,97 @@
+// TU: coverage test and launches of the tensor-core (wgmma) kernel family (vil_wgmma.cuh).  The global query rows, the
+// global key columns of the backward and delta = rowsum(dO * O) come from the shared SIMT kernels (vil_simt.cu).
+#include <cstdio>
+#include "vil_host.cuh"
+#include "vil_wgmma.cuh"
+
+namespace vil {
+namespace {
+
+int head_tile(int D) { return D <= 16 ? 16 : D <= 32 ? 32 : 64; }
+int table_floats(const Geo& g) { return g.has_bias ? (4 * g.w - 1) * (4 * g.w - 1) : 0; }
+
+template <typename K>
+int set_smem(K kernel, size_t bytes) {
+  if (bytes > 227 * 1024) return shared_fail(VIL_E_UNSUPPORTED, "configuration needs more than 227 KB of shared memory");
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e != cudaSuccess) return shared_fail(VIL_E_CUDA, cudaGetErrorString(e));
+  return VIL_OK;
+}
+
+const char* why_not(const VilAttnParams* p, const Geo& g) {
+  if (p->dtype != VIL_BF16 && p->dtype != VIL_F16) return "dtype is fp32 (wgmma operands are bf16 / fp16)";
+  if (g.D > 64) return "head dim > 64";
+  if (wg::DkvSmem<64>::total(table_floats(g)) > 227 * 1024) return "bias table does not fit in shared memory";
+  return nullptr;
+}
+
+long long blocks(const Geo& g) { return (long long)g.B * g.H * g.mx * g.my * g.npc; }
+
+template <typename T, int HD, typename TO>
+int forward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+  int rc;
+  if (!(p->skip_mask & 2)) {
+    const size_t sm = wg::FwdSmem<HD>::total(table_floats(g));
+    if ((rc = set_smem(wg::wg_fwd_local<T, HD, TO>, sm))) return rc;
+    wg::wg_fwd_local<T, HD, TO><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse,
+                                                                            p->bias_table, p->g2l);
+    count_launch();
+    if ((rc = launch_check("wgmma_fwd_local"))) return rc;
+  }
+  if (g.g > 0 && !(p->skip_mask & 1)) return simt_global_fwd(p, g, s);
+  return VIL_OK;
+}
+
+template <typename T, int HD, typename TO>
+int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+  int rc;
+  if (!(p->skip_mask & 8) && (rc = simt_delta(p, g, s))) return rc;
+  float* delta = static_cast<float*>(p->workspace);
+  const int tabn = table_floats(g);
+  if (!(p->skip_mask & 2)) {
+    const size_t sm = wg::DqSmem<HD>::total(tabn);
+    if ((rc = set_smem(wg::wg_bwd_dq<T, HD, TO>, sm))) return rc;
+    wg::wg_bwd_dq<T, HD, TO><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq),
+                                                                         p->lse, delta, p->bias_table, p->g2l, p->d_bias_table);
+    count_launch();
+    if ((rc = launch_check("wgmma_bwd_dq"))) return rc;
+  }
+  if (!(p->skip_mask & 4)) {
+    const size_t sm = wg::DkvSmem<HD>::total(tabn);
+    if ((rc = set_smem(wg::wg_bwd_dkv<T, HD, TO>, sm))) return rc;
+    wg::wg_bwd_dkv<T, HD, TO><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk),
+                                                                          t4(p->dv), p->lse, delta, p->bias_table);
+    count_launch();
+    if ((rc = launch_check("wgmma_bwd_dkv"))) return rc;
+  }
+  if (g.g > 0 && !(p->skip_mask & 1)) return simt_global_bwd(p, g, s, g.N);
+  return VIL_OK;
+}
+
+template <typename T, typename TO>
+int dispatch_hd(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
+  switch (head_tile(g.D)) {
+    case 16: return bwd ? backward_t<T, 16, TO>(p, g, s) : forward_t<T, 16, TO>(p, g, s);
+    case 32: return bwd ? backward_t<T, 32, TO>(p, g, s) : forward_t<T, 32, TO>(p, g, s);
+    default: return bwd ? backward_t<T, 64, TO>(p, g, s) : forward_t<T, 64, TO>(p, g, s);
+  }
+}
+
+int run(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
+  note_kernel(bwd ? "wgmma_bwd" : "wgmma_fwd");
+  if (p->dtype == VIL_BF16)
+    return out_f32(p) ? dispatch_hd<__nv_bfloat16, float>(p, g, s, bwd) : dispatch_hd<__nv_bfloat16, __nv_bfloat16>(p, g, s, bwd);
+  return out_f32(p) ? dispatch_hd<__half, float>(p, g, s, bwd) : dispatch_hd<__half, __half>(p, g, s, bwd);
+}
+
+}  // namespace
+
+const char* tc_why_not(const VilAttnParams* p, const Geo& g, bool) {
+  const char* w = why_not(p, g);
+  return w ? w : "supported";
+}
+int tc_supported(const VilAttnParams* p, const Geo& g, bool) { return why_not(p, g) == nullptr; }
+int tc_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) { return run(p, g, s, false); }
+int tc_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) { return run(p, g, s, true); }
+
+}  // namespace vil

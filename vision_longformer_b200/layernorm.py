@@ -84,7 +84,7 @@ class _FusedLayerNorm(torch.autograd.Function):
 
 
 class B200LayerNorm(nn.LayerNorm):
-    """Drop-in `nn.LayerNorm` (last-dim, affine) backed by the sm_100a kernels.  `keep_dtype=True` marks a norm whose
+    """Drop-in `nn.LayerNorm` (last-dim, affine) backed by the sm_90a kernels.  `keep_dtype=True` marks a norm whose
     output joins the fp32 residual stream (the patch-embedding norm): an fp32 input stays fp32 even under autocast,
     and a bf16/fp16 input under autocast (the Conv2d output) is normalised into an fp32 result by the low-precision-in ->
     fp32-out kernel variant - the dtype `nn.LayerNorm` gives the reference there (autocast runs layer_norm in fp32), in

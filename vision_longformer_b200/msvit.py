@@ -117,16 +117,15 @@ class DenseAttention(nn.Module):
     """Full multi-head attention of the `s0` stages with optional Swin-style relative bias and global-token biases
     (reference `Attention`, msvit.py:37-120).
 
-    impl = "vil"  : the vil_attn sm_100a kernels - dense attention over nglo + w*w tokens is the SINGLE-CHUNK case of the
+    impl = "vil"  : the vil_attn sm_90a kernels - dense attention over nglo + w*w tokens is the SINGLE-CHUNK case of the
                     sliding-chunk operator (nx = ny = w, every local query sees every local key, global tokens as usual),
-                    so the same tcgen05 kernels serve it when w in {7, 14} (7x7 and 14x14 stages of the 224 nets),
+                    so the same tensor-core kernels serve it when w in {7, 14} (7x7 and 14x14 stages of the 224 nets),
                     head dim <= 64, bf16/fp16 on CUDA; no (H,N,N) bias tensor is materialised: the Swin-style
                     (2wx-1)(2wy-1) table is embedded in the operator's (4w-1)^2 index space (same Delta-row / Delta-col).
     impl = "sdpa" : stock F.scaled_dot_product_attention (cuDNN) with the bias as attn_mask.
-    impl = "auto" : "sdpa".  MEASURED on B200 (profiles/r02_time_dense.log, B=256, bf16, module fwd+bwd): 14x14+1 tokens
-                    1.32 ms (vil) vs 0.91 ms (cuDNN); 7x7 tokens 0.90 vs 0.71 ms - at 50..197 tokens the chunk-tiled kernels
-                    (64-row slots, one global-token side kernel, two backward passes) lose to a dedicated dense flash kernel,
-                    so the faster library path stays the default and "vil" is opt-in (parity-tested in
+    impl = "auto" : "sdpa": at 50..197 tokens the chunk-tiled kernels (64-row tiles, one global-token side kernel, two
+                    backward passes) are not expected to beat a dedicated dense flash kernel (tools/time_dense.py times both),
+                    so the library path stays the default and "vil" is opt-in (parity-tested in
                     tests/test_gpu_parity.py::test_dense_attention_on_the_operator_kernels)."""
 
     supports_deferred_bias = True       # forward(..., defer_proj_bias=True) -> (projection without bias, bias)
@@ -370,7 +369,7 @@ class MsViT(nn.Module):
         # LayerNorm it builds comes from the `norm_layer` ARGUMENT, whose default eps is 1e-6 (msvit.py:350,
         # 356-361, 378-390, 436).  LN_EPS therefore has no effect there; mirrored here for parity.
         del ln_eps
-        # fused_norm: nn.LayerNorm subclass backed by the sm_100a LayerNorm kernels (SURVEY.md section 8 (f) row 4);
+        # fused_norm: nn.LayerNorm subclass backed by the sm_90a LayerNorm kernels (SURVEY.md section 8 (f) row 4);
         # same parameters / state_dict, falls back to nn.LayerNorm on CPU.  The patch-embedding norm keeps its
         # input dtype because its output becomes the fp32 residual stream.
         # fused_residual: residual add + DropPath scale + deferred Linear bias + LayerNorm in one kernel per block boundary,

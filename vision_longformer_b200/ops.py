@@ -21,13 +21,13 @@ from . import _lib
 from ._lib import VilAttnParams, VilTensor4
 
 _DTYPES = {torch.float32: _lib.VIL_F32, torch.bfloat16: _lib.VIL_BF16, torch.float16: _lib.VIL_F16}
-_IMPLS = {"auto": _lib.VIL_IMPL_AUTO, "simt": _lib.VIL_IMPL_SIMT, "tcgen05": _lib.VIL_IMPL_TCGEN05}
+_IMPLS = {"auto": _lib.VIL_IMPL_AUTO, "simt": _lib.VIL_IMPL_SIMT, "wgmma": _lib.VIL_IMPL_WGMMA}
 
 
 def _require_cuda(t: torch.Tensor, name: str):
     if not t.is_cuda:
         raise RuntimeError(
-            f"vil_attention: `{name}` is on {t.device}; this operator only runs on a CUDA (sm_100a) device - "
+            f"vil_attention: `{name}` is on {t.device}; this operator only runs on a CUDA (sm_90a) device - "
             "there is no CPU fallback")
 
 
@@ -224,7 +224,7 @@ def vil_attention(q_all, kv, qg_all=None, kvg=None, table=None, g2l=None, g2g=No
 
     Under `torch.autocast('cuda')` the activations are cast to the autocast dtype first (the reference's
     `@autocast()`-decorated SlidingChunk2D does the same, slidingchunk_2d.py:203,235), so an fp32 caller gets the
-    tcgen05 path and bf16/fp16 outputs; the bias tables stay fp32.
+    tensor-core path and bf16/fp16 outputs; the bias tables stay fp32.
     """
     if q_all.is_cuda and torch.is_autocast_enabled("cuda"):
         dt = torch.get_autocast_dtype("cuda")
