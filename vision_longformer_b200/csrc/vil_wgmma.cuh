@@ -2,7 +2,8 @@
 //
 // Same decomposition and masking rules as the SIMT family (vil_simt.cuh), with every product on the tensor cores:
 // a CTA is one warpgroup (128 threads) owning a 64-row tile; it walks 64-column pieces (the global keys, then the
-// visited chunks piece by piece).  Per piece the operands are staged into shared memory as 8x8 core matrices and
+// visited chunks piece by piece).  Per piece the operands are staged into shared memory as 8x8 core matrices, with the
+// mask / bias terms of every column, and
 //   forward          S = Q K^T (SS), online softmax in registers, O += P V (RS: P stays in registers)
 //   backward pass 1  S = Q K^T, dP = dO V^T (SS), dS = P (dP - delta), dQ += dS K (RS)         (query-stationary)
 //   backward pass 2  S^T = K Q^T, dP^T = V dO^T (SS), dV += P^T dO, dK += dS^T Q (RS)           (key-stationary)
@@ -75,74 +76,189 @@ __device__ __forceinline__ void store_rows(const float (&acc)[HD / 2], int e, TO
   }
 }
 
-// One piece of <= 64 keys visible from query chunk (R, C): which tokens, which flags (0 none, 1 local, 2 global) and the
-// (row, column) of every key relative to the query chunk's origin -- the rules of simt_fwd_local.
-struct KeyPieces {
-  int ngp, n;
-  __device__ KeyPieces(const Geo& g) : ngp((g.g + 63) / 64), n((g.g + 63) / 64 + g.noffs * g.npc) {}
+// The walk.  A CTA lists the chunks it visits once, in shared memory: chunks outside the image are dropped (wrapped when
+// exact == -1), the rest kept in offset order.  The forward and pass 1 take ceil(g / 64) pieces of global keys, then npc
+// pieces per visited chunk; pass 2 takes npc query pieces per chunk that visits its keys.  Each chunk starts a piece of
+// its own: the grouping of keys into pieces fixes the order of the fp32 sums of O, dQ, dK and dV and the running max that
+// P is rounded against, and with it the bits of every result.
+struct Visit {
+  int r, c;     // the visited chunk
+  int dR, dC;   // its offset (key chunk = query chunk + offset)
+  int cut;      // exact == -1: bit 0 / 1 = the query chunk + offset is the last chunk row / column (its padded keys are cut)
 };
-// returns false when the piece lies outside the image (CTA-uniform skip)
-__device__ __forceinline__ bool key_piece(const Geo& geo, int R, int C, int pi, int ngp, int slot, long long& tok, int& flag,
-                                          int& vr, int& vc) {
-  tok = -1; flag = 0; vr = 0; vc = 0;
-  const int w = geo.w;
-  if (pi < ngp) {
-    const int t = pi * 64 + slot;
-    if (t < geo.g) { flag = 2; vr = t; tok = t; }
-    return true;
+
+// sgn = +1: the key chunks seen by query chunk (R, C); sgn = -1: the query chunks that see key chunk (R, C)
+__device__ __forceinline__ int visit_list(const Geo& geo, int R, int C, int sgn, Visit* vl) {
+  int n = 0;
+  for (int oi = 0; oi < geo.noffs; ++oi) {
+    const int dR = geo.offR[oi], dC = geo.offC[oi];
+    int r = R + sgn * dR, c = C + sgn * dC;
+    if (geo.exact == -1) { r = (r + geo.mx) % geo.mx; c = (c + geo.my) % geo.my; }
+    else if (r < 0 || r >= geo.mx || c < 0 || c >= geo.my) continue;
+    const int qR = sgn > 0 ? R : r, qC = sgn > 0 ? C : c;
+    if (threadIdx.x == 0) vl[n] = Visit{r, c, dR, dC, (qR + dR == geo.mx - 1) | ((qC + dC == geo.my - 1) << 1)};
+    ++n;
   }
-  const int oi = (pi - ngp) / geo.npc, kp = (pi - ngp) % geo.npc;
-  const int dR = geo.offR[oi], dC = geo.offC[oi];
-  int KR = R + dR, KC = C + dC;
-  if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
-  else if (KR < 0 || KR >= geo.mx || KC < 0 || KC >= geo.my) return false;
-  const int lk = kp * 64 + slot;
-  if (lk < geo.w2) {
-    const int kr = lk / w, kc = lk % w;
-    const int ar = KR * w + kr, ac = KC * w + kc;
-    const bool real = (ar < geo.nx) && (ac < geo.ny);
-    if (geo.exact == -1)
-      flag = !(((R + dR == geo.mx - 1) && (kr >= w - geo.padx)) || ((C + dC == geo.my - 1) && (kc >= w - geo.pady)));
-    else
-      flag = real;
-    if (flag && real) tok = geo.g + (long long)ar * geo.ny + ac;   // phantom padding keys keep K = V = 0
-    vr = dR * w + kr; vc = dC * w + kc;
-  }
-  return true;
+  return n;
 }
 
-// additive bias of (query row qr, qc) against key j; false when the pair is masked
-__device__ __forceinline__ bool pair_bias(const Geo& geo, int f, int kvr, int kvc, int qr, int qc, int h, const float* tab,
-                                          const float* __restrict__ g2l, float& bias, int& bidx) {
-  bias = 0.f; bidx = -1;
-  if (f == 2) {
-    if (geo.has_bias) bias = g2l[((long long)geo.H + h) * geo.g + kvr];
-    return true;
+// Key lk (< w^2) of visited chunk v: the token (-1: a zero row), whether the column takes part at all (the pad-cut rule
+// folded in), and the key's (row, column) relative to the query chunk's origin -- the rules of simt_fwd_local.
+__device__ __forceinline__ void chunk_key(const Geo& geo, const Visit& v, int lk, long long& tok, bool& ok, int& vr, int& vc) {
+  const int w = geo.w, kr = lk / w, kc = lk - kr * w;
+  const int ar = v.r * w + kr, ac = v.c * w + kc;
+  const bool real = (ar < geo.nx) && (ac < geo.ny);
+  if (geo.exact == -1)
+    ok = !(((v.cut & 1) && (kr >= w - geo.padx)) || ((v.cut & 2) && (kc >= w - geo.pady)));
+  else
+    ok = real;
+  tok = (ok && real) ? geo.g + (long long)ar * geo.ny + ac : -1;   // phantom padding keys keep K = V = 0
+  vr = v.dR * w + kr; vc = v.dC * w + kc;
+}
+
+// Column slot of key piece pi (ngp pieces of global keys, then npc per visited chunk): gk = the global key (-1 for a
+// local one or an empty slot), then as chunk_key.  Global keys sit at (0, 0), which every query of the chunk sees under
+// the exact window.
+__device__ __forceinline__ void key_slot(const Geo& geo, const Visit* vl, int ngp, int pi, int slot, int& gk, long long& tok,
+                                         bool& ok, int& vr, int& vc) {
+  gk = -1; tok = -1; ok = false; vr = 0; vc = 0;
+  if (pi < ngp) {
+    const int t = pi * 64 + slot;
+    if (t < geo.g) { gk = t; tok = t; ok = true; }
+    return;
   }
-  const int w = geo.w, dr = qr - kvr, dc = qc - kvc;
-  if (geo.exact == 1 && (abs(dr) > w || abs(dc) > w)) return false;
-  if (geo.has_bias) { bidx = (dr + 2 * w - 1) * (4 * w - 1) + dc + 2 * w - 1; bias = tab[bidx]; }
-  return true;
+  const int vi = (pi - ngp) / geo.npc, lk = (pi - ngp - vi * geo.npc) * 64 + slot;
+  if (lk < geo.w2) chunk_key(geo, vl[vi], lk, tok, ok, vr, vc);
+}
+
+// Per-column metadata of a staged key piece, written once per round.  The score of (query row, key column j) is
+// scale * s + bias[j] (+ tab[row base - tix[j]] with the bias table), -inf where bias[j] = -inf or the exact window
+// |qr - kr[j]|, |qc - kc[j]| <= w fails.
+struct KeyCols {
+  float* bias;   // 0, the global key's g2l bias, or -inf for a masked column
+  int* tix;      // bias-table offset of the key: kr * (4w - 1) + kc
+  short* kr;
+  short* kc;
+};
+// query row of the 64-row tile: chunk-relative position (0 for rows past the chunk, which are computed and dropped)
+struct QRows {
+  int qr[2], qc[2];
+  bool ok[2];
+};
+
+__device__ __forceinline__ QRows query_rows(const Geo& geo, int R, int C, int piece) {
+  QRows q;
+  const int w = geo.w;
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int l = piece * 64 + acc_row(2 * e);
+    const bool in = l < geo.w2;
+    q.qr[e] = in ? l / w : 0; q.qc[e] = in ? l % w : 0;
+    q.ok[e] = in && (R * w + q.qr[e] < geo.nx) && (C * w + q.qc[e] < geo.ny);
+  }
+  return q;
+}
+
+__device__ __forceinline__ void stage_key_cols(const Geo& geo, const KeyCols& kc, int h, const float* __restrict__ g2l, int gk,
+                                               bool ok, int vr, int vc) {
+  const int slot = threadIdx.x >> 1;
+  float bias = ok ? 0.f : -INFINITY;
+  if (gk >= 0 && geo.has_bias) bias = g2l[((long long)geo.H + h) * geo.g + gk];
+  kc.bias[slot] = bias;
+  kc.tix[slot] = vr * (4 * geo.w - 1) + vc;
+  kc.kr[slot] = (short)vr;
+  kc.kc[slot] = (short)vc;
+}
+
+// bias-table offset of the query rows (dr = dc = 0 at the table's centre): the entry of a pair is tb - KeyCols::tix
+__device__ __forceinline__ void row_tix(const Geo& geo, const QRows& q, int (&tb)[2]) {
+  const int w = geo.w, tw = 4 * w - 1;
+  tb[0] = (q.qr[0] + 2 * w - 1) * tw + q.qc[0] + 2 * w - 1;
+  tb[1] = (q.qr[1] + 2 * w - 1) * tw + q.qc[1] + 2 * w - 1;
+}
+
+// Masked, biased score of accumulator element s (row e of the thread, key column j); bidx = the bias-table entry it used
+// (-1 for a global key or without the table).  gl = g - 64 * piece: columns j < gl are global keys.
+template <bool RPE, bool WIN>
+__device__ __forceinline__ float key_score(const Geo& geo, const KeyCols& kc, const float* tab, const QRows& q, const int (&tb)[2],
+                                           int e, int j, int gl, float s, int& bidx) {
+  float bias = kc.bias[j];
+  bidx = -1;
+  if (RPE && j >= gl) { bidx = tb[e] - kc.tix[j]; bias += tab[bidx]; }
+  if (WIN && (abs(q.qr[e] - kc.kr[j]) > geo.w || abs(q.qc[e] - kc.kc[j]) > geo.w)) return -INFINITY;
+  return fmaf(geo.scale, s, bias);
+}
+
+// Score epilogue: which of the four per-element forms a CTA runs, chosen once from the call's configuration
+__device__ __forceinline__ int key_epilogue(const Geo& geo) { return (geo.has_bias ? 2 : 0) | (geo.exact == 1 ? 1 : 0); }
+
+// forward: scores of one piece and their row maxima
+template <bool RPE, bool WIN>
+__device__ __forceinline__ void fwd_scores(float (&s)[32], float (&mx)[2], const Geo& geo, const KeyCols& kc, const float* tab,
+                                           const QRows& q, int gl) {
+  int tb[2] = {0, 0};
+  if (RPE) row_tix(geo, q, tb);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const int e = (i >> 1) & 1;
+    int bidx;
+    s[i] = key_score<RPE, WIN>(geo, kc, tab, q, tb, e, acc_col(i), gl, s[i], bidx);
+    mx[e] = fmaxf(mx[e], s[i]);
+  }
+}
+
+// pass 1: dS = P (dP - delta) of one piece into s, and the bias-table gradient when d_table is set.  Rows past the chunk
+// carry lse = +inf, so their P is 0.
+template <bool RPE, bool WIN>
+__device__ __forceinline__ void dq_scores(float (&s)[32], const float (&dp)[32], const Geo& geo, const KeyCols& kc,
+                                          const float* tab, const QRows& q, int gl, const float (&lse_r)[2],
+                                          const float (&del_r)[2], float* __restrict__ d_table, int h) {
+  int tb[2] = {0, 0};
+  if (RPE) row_tix(geo, q, tb);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const int e = (i >> 1) & 1;
+    int bidx;
+    const float val = key_score<RPE, WIN>(geo, kc, tab, q, tb, e, acc_col(i), gl, s[i], bidx);
+    const float ds = __expf(val - lse_r[e]) * (dp[i] - del_r[e]);
+    if (RPE && d_table != nullptr && bidx >= 0 && q.ok[e] && val != -INFINITY)
+      atomicAdd(d_table + (long long)bidx * geo.H + h, ds);
+    s[i] = ds;
+  }
+}
+
+constexpr size_t kKeyMeta = 64 * (4 + 4 + 2 + 2) + 9 * sizeof(Visit);
+constexpr size_t kQueryMeta = 64 * (4 + 4 + 4 + 2 + 2 + 1) + 9 * sizeof(Visit);
+
+__device__ __forceinline__ KeyCols key_cols(float* base, Visit*& vl) {
+  KeyCols kc;
+  kc.bias = base;
+  kc.tix = reinterpret_cast<int*>(kc.bias + 64);
+  vl = reinterpret_cast<Visit*>(kc.tix + 64);
+  kc.kr = reinterpret_cast<short*>(vl + 9);
+  kc.kc = kc.kr + 64;
+  return kc;
 }
 
 template <int HD> struct FwdSmem {
   static constexpr size_t tiles = 3 * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + 64 * 5 + 15) & ~size_t(15); }
+  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + kKeyMeta + 15) & ~size_t(15); }
 };
 template <int HD> struct DqSmem {
   static constexpr size_t tiles = 5 * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + 64 * 5 + 15) & ~size_t(15); }
+  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + kKeyMeta + 15) & ~size_t(15); }
 };
 template <int HD> struct DkvSmem {
   static constexpr size_t tiles = 6 * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + 64 * 13 + 15) & ~size_t(15); }
+  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + kQueryMeta + 15) & ~size_t(15); }
 };
 
 // ----------------------------------------------------------------------------------------------
 // forward, local queries
 // ----------------------------------------------------------------------------------------------
+// held to 5 / 3 CTAs per SM (HD <= 32 / 64): left alone, ptxas spends registers on hoisting the column loads and drops one
 template <typename T, int HD, typename TO>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, HD <= 32 ? 5 : 3)
 wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const float* __restrict__ table,
              const float* __restrict__ g2l) {
   constexpr int HH = HD / 2;
@@ -153,11 +269,9 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   T* Ks = Qs + 64 * HD;
   T* Vt = Ks + 64 * HD;
   float* tab = reinterpret_cast<float*>(Vt + 64 * HD);
-  const int tw = 4 * geo.w - 1;
-  const int tabn = geo.has_bias ? tw * tw : 0;
-  short* kvr = reinterpret_cast<short*>(tab + tabn);
-  short* kvc = kvr + 64;
-  unsigned char* kfl = reinterpret_cast<unsigned char*>(kvc + 64);
+  const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
+  Visit* vl;
+  const KeyCols kcol = key_cols(tab + tabn, vl);
 
   const Cta cid = decode(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
@@ -173,25 +287,20 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     if (l < geo.w2 && r < geo.nx && c < geo.ny) load_seg<T, HH>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), half * HH, D, x);
     stage_half_row<T, HD>(Qs, nullptr, x, slot, half);
   }
-  int qr[2], qc[2];
-  bool qok[2];
-#pragma unroll
-  for (int e = 0; e < 2; ++e) {
-    const int l = cid.piece * 64 + acc_row(2 * e);
-    qr[e] = l / w; qc[e] = l % w;
-    qok[e] = (l < geo.w2) && (R * w + qr[e] < geo.nx) && (C * w + qc[e] < geo.ny);
-  }
   float m[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
   float oacc[HH];
 #pragma unroll
   for (int i = 0; i < HH; ++i) oacc[i] = 0.f;
 
-  const KeyPieces kp(geo);
-  for (int pi = 0; pi < kp.n; ++pi) {
-    long long tok; int flag, vr, vc;
-    if (!key_piece(geo, R, C, pi, kp.ngp, slot, tok, flag, vr, vc)) continue;   // CTA-uniform
+  const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, R, C, 1, vl) * geo.npc;
+  const int epi = key_epilogue(geo);
+  for (int pi = 0; pi < npieces; ++pi) {
     __syncthreads();
     {
+      int gk, vr, vc;
+      long long tok;
+      bool ok;
+      key_slot(geo, vl, ngp, pi, slot, gk, tok, ok, vr, vc);
       float kk[HH], vv[HH];
 #pragma unroll
       for (int i = 0; i < HH; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
@@ -202,7 +311,7 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
       stage_half_row<T, HD>(Ks, nullptr, kk, slot, half);
 #pragma unroll
       for (int i = 0; i < HH; ++i) Vt[sm90::core_off(half * HH + i, slot, 64)] = ElemTraits<T>::from_f(vv[i]);
-      if (half == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
+      if (half == 0) stage_key_cols(geo, kcol, h, g2l, gk, ok, vr, vc);
     }
     sm90::fence_proxy_async();
     __syncthreads();
@@ -214,14 +323,13 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     sm90::wg_wait0();
     sm90::reg_fence(s);
     float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int e = (i >> 1) & 1, j = acc_col(i), f = kfl[j];
-      float val = -INFINITY, bias;
-      int bidx;
-      if (f && qok[e] && pair_bias(geo, f, kvr[j], kvc[j], qr[e], qc[e], h, tab, g2l, bias, bidx)) val = fmaf(geo.scale, s[i], bias);
-      s[i] = val;
-      mx[e] = fmaxf(mx[e], val);
+    const int gl = geo.g - pi * 64;
+    // the row coordinates are derived where they are used: kept live across the loop, they cost the HD 32 forward a spill
+    switch (epi) {   // CTA-uniform
+      case 0: fwd_scores<false, false>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
+      case 1: fwd_scores<false, true>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
+      case 2: fwd_scores<true, false>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
+      default: fwd_scores<true, true>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
     }
     float corr[2];
 #pragma unroll
@@ -252,12 +360,13 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     sm90::wg_wait0();
     sm90::reg_fence(oacc);
   }
+  const QRows qrow = query_rows(geo, R, C, cid.piece);
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     lsum[e] += __shfl_xor_sync(0xffffffffu, lsum[e], 1);
     lsum[e] += __shfl_xor_sync(0xffffffffu, lsum[e], 2);
-    if (!qok[e]) continue;
-    const long long tokq = (long long)(R * w + qr[e]) * geo.ny + (C * w + qc[e]);
+    if (!qrow.ok[e]) continue;
+    const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
     store_rows<TO, HD>(oacc, e, row_ptr_w<TO>(o, b, h, tokq), D, lsum[e] > 0.f ? 1.f / lsum[e] : 0.f);
     if ((tid & 3) == 0) lse[((long long)b * geo.H + h) * geo.Nloc + tokq] = m[e] + logf(lsum[e]);
   }
@@ -280,11 +389,9 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   T* Vs = Ks + 64 * HD;
   T* Kt = Vs + 64 * HD;
   float* tab = reinterpret_cast<float*>(Kt + 64 * HD);
-  const int tw = 4 * geo.w - 1;
-  const int tabn = geo.has_bias ? tw * tw : 0;
-  short* kvr = reinterpret_cast<short*>(tab + tabn);
-  short* kvc = kvr + 64;
-  unsigned char* kfl = reinterpret_cast<unsigned char*>(kvc + 64);
+  const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
+  Visit* vl;
+  const KeyCols kcol = key_cols(tab + tabn, vl);
 
   const Cta cid = decode(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
@@ -305,17 +412,13 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     stage_half_row<T, HD>(Qs, nullptr, x, slot, half);
     stage_half_row<T, HD>(Gs, nullptr, y, slot, half);
   }
-  int qr[2], qc[2];
-  bool qok[2];
+  const QRows qrow = query_rows(geo, R, C, cid.piece);
   float lse_r[2], del_r[2];
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
-    const int l = cid.piece * 64 + acc_row(2 * e);
-    qr[e] = l / w; qc[e] = l % w;
-    qok[e] = (l < geo.w2) && (R * w + qr[e] < geo.nx) && (C * w + qc[e] < geo.ny);
     lse_r[e] = INFINITY; del_r[e] = 0.f;
-    if (qok[e]) {
-      const long long tokq = (long long)(R * w + qr[e]) * geo.ny + (C * w + qc[e]);
+    if (qrow.ok[e]) {
+      const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
       lse_r[e] = lse[bh * geo.Nloc + tokq];
       del_r[e] = delta[bh * geo.Nloc + tokq];
     }
@@ -324,12 +427,15 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
 #pragma unroll
   for (int i = 0; i < HH; ++i) dqacc[i] = 0.f;
 
-  const KeyPieces kp(geo);
-  for (int pi = 0; pi < kp.n; ++pi) {
-    long long tok; int flag, vr, vc;
-    if (!key_piece(geo, R, C, pi, kp.ngp, slot, tok, flag, vr, vc)) continue;
+  const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, R, C, 1, vl) * geo.npc;
+  const int epi = key_epilogue(geo);
+  for (int pi = 0; pi < npieces; ++pi) {
     __syncthreads();
     {
+      int gk, vr, vc;
+      long long tok;
+      bool ok;
+      key_slot(geo, vl, ngp, pi, slot, gk, tok, ok, vr, vc);
       float kk[HH], vv[HH];
 #pragma unroll
       for (int i = 0; i < HH; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
@@ -339,7 +445,7 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
       }
       stage_half_row<T, HD>(Ks, Kt, kk, slot, half);
       stage_half_row<T, HD>(Vs, nullptr, vv, slot, half);
-      if (half == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
+      if (half == 0) stage_key_cols(geo, kcol, h, g2l, gk, ok, vr, vc);
     }
     sm90::fence_proxy_async();
     __syncthreads();
@@ -353,17 +459,12 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     sm90::wg_wait0();
     sm90::reg_fence(s);
     sm90::reg_fence(dp);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int e = (i >> 1) & 1, j = acc_col(i), f = kfl[j];
-      float ds = 0.f, bias;
-      int bidx;
-      if (f && qok[e] && pair_bias(geo, f, kvr[j], kvc[j], qr[e], qc[e], h, tab, g2l, bias, bidx)) {
-        const float p = __expf(fmaf(geo.scale, s[i], bias) - lse_r[e]);
-        ds = p * (dp[i] - del_r[e]);
-        if (bidx >= 0 && d_table != nullptr) atomicAdd(d_table + (long long)bidx * geo.H + h, ds);
-      }
-      s[i] = ds;
+    const int gl = geo.g - pi * 64;
+    switch (epi) {   // CTA-uniform
+      case 0: dq_scores<false, false>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
+      case 1: dq_scores<false, true>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
+      case 2: dq_scores<true, false>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
+      default: dq_scores<true, true>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
     }
     uint32_t a[4][4];
 #pragma unroll
@@ -377,8 +478,8 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   }
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
-    if (!qok[e]) continue;
-    const long long tokq = (long long)(R * w + qr[e]) * geo.ny + (C * w + qc[e]);
+    if (!qrow.ok[e]) continue;
+    const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
     store_rows<TO, HD>(dqacc, e, row_ptr_w<TO>(dq, b, h, tokq), D, geo.scale);
   }
 }
@@ -387,6 +488,58 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
 // backward pass 2 (key-stationary): dk, dv of the LOCAL key rows.  CTA = one 64-key piece of one key chunk; it walks the
 // query chunks that visit it (the symmetric image of the offset list), 64 queries at a time.
 // ----------------------------------------------------------------------------------------------
+
+// Per-column metadata of a staged query piece.  With (qr, qc) = the query's position minus offset * w, the pair with key
+// row (kr, kc) of the key chunk has dr = qr - kr, dc = qc - kc.
+struct QueryCols {
+  float* lse;            // +inf for a column without a real query, so that its P is 0
+  float* del;
+  int* tix;              // bias-table offset: qr * (4w - 1) + qc
+  short* qr;
+  short* qc;
+  unsigned char* cut;    // Visit::cut of the query's chunk
+};
+// key row of the 64-row tile (0 for rows past the chunk, which are computed and dropped)
+struct KRows {
+  int kr[2], kc[2], tb[2];   // tb: bias entry of the pair = tix[j] - tb
+  int cut[2];                // exact == -1: bit 0 / 1 = the key lies in the padded rows / columns of its chunk
+  bool real[2];
+};
+
+__device__ __forceinline__ QueryCols query_cols(float* base, Visit*& vl) {
+  QueryCols qc;
+  qc.lse = base;
+  qc.del = qc.lse + 64;
+  qc.tix = reinterpret_cast<int*>(qc.del + 64);
+  vl = reinterpret_cast<Visit*>(qc.tix + 64);
+  qc.qr = reinterpret_cast<short*>(vl + 9);
+  qc.qc = qc.qr + 64;
+  qc.cut = reinterpret_cast<unsigned char*>(qc.qc + 64);
+  return qc;
+}
+
+// Pass 2's per-element forms: RPE adds the bias table, MASK 1 is the exact window (exact == 1), MASK 2 the pad cut of
+// exact == -1
+__device__ __forceinline__ int query_epilogue(const Geo& geo) {
+  return (geo.has_bias ? 3 : 0) + (geo.exact == 1 ? 1 : geo.exact == -1 ? 2 : 0);
+}
+
+// P^T into s and dS^T into dp for one query piece
+template <bool RPE, int MASK>
+__device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const Geo& geo, const QueryCols& qc, const float* tab,
+                                          const KRows& kr) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const int e = (i >> 1) & 1, j = acc_col(i);
+    float x = fmaf(geo.scale, s[i], RPE ? tab[qc.tix[j] - kr.tb[e]] : 0.f) - qc.lse[j];
+    if (MASK == 1 && (abs(qc.qr[j] - kr.kr[e]) > geo.w || abs(qc.qc[j] - kr.kc[e]) > geo.w)) x = -INFINITY;
+    if (MASK == 2 && (qc.cut[j] & kr.cut[e])) x = -INFINITY;
+    const float p = __expf(x);
+    s[i] = p;
+    dp[i] = p * (dp[i] - qc.del[j]);
+  }
+}
+
 template <typename T, int HD, typename TO>
 __global__ void __launch_bounds__(kThreads)
 wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse, const float* __restrict__ delta,
@@ -404,11 +557,8 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
   float* tab = reinterpret_cast<float*>(Gt + 64 * HD);
   const int tw = 4 * geo.w - 1;
   const int tabn = geo.has_bias ? tw * tw : 0;
-  float* lse_s = tab + tabn;
-  float* del_s = lse_s + 64;
-  short* qrs = reinterpret_cast<short*>(del_s + 64);
-  short* qcs = qrs + 64;
-  unsigned char* qfl = reinterpret_cast<unsigned char*>(qcs + 64);
+  Visit* vl;
+  const QueryCols qcol = query_cols(tab + tabn, vl);
 
   const Cta cid = decode(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, KR = cid.R, KC = cid.C;
@@ -430,98 +580,91 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     stage_half_row<T, HD>(Ks, nullptr, x, slot, half);
     stage_half_row<T, HD>(Vs, nullptr, y, slot, half);
   }
-  int kr[2], kc[2];
-  bool kreal[2];
+  KRows krow;
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     const int lk = cid.piece * 64 + acc_row(2 * e);
-    kr[e] = lk / w; kc[e] = lk % w;
-    kreal[e] = (lk < geo.w2) && (KR * w + kr[e] < geo.nx) && (KC * w + kc[e] < geo.ny);
+    const bool in = lk < geo.w2;
+    krow.kr[e] = in ? lk / w : 0; krow.kc[e] = in ? lk % w : 0;
+    krow.real[e] = in && (KR * w + krow.kr[e] < geo.nx) && (KC * w + krow.kc[e] < geo.ny);
+    krow.tb[e] = krow.kr[e] * tw + krow.kc[e] - (2 * w - 1) * (tw + 1);
+    krow.cut[e] = (krow.kr[e] >= w - geo.padx) | ((krow.kc[e] >= w - geo.pady) << 1);
   }
   float dkacc[HH], dvacc[HH];
 #pragma unroll
   for (int i = 0; i < HH; ++i) { dkacc[i] = 0.f; dvacc[i] = 0.f; }
 
-  for (int oi = 0; oi < geo.noffs; ++oi) {
-    const int dR = geo.offR[oi], dC = geo.offC[oi];
-    int QR = KR - dR, QC = KC - dC;
-    if (geo.exact == -1) { QR = (QR + geo.mx) % geo.mx; QC = (QC + geo.my) % geo.my; }
-    else if (QR < 0 || QR >= geo.mx || QC < 0 || QC >= geo.my) continue;
-    bool kvis[2];
-    int vr[2], vc[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      kvis[e] = kreal[e];
-      if (geo.exact == -1)
-        kvis[e] = kreal[e] && !(((QR + dR == geo.mx - 1) && (kr[e] >= w - geo.padx)) ||
-                                ((QC + dC == geo.my - 1) && (kc[e] >= w - geo.pady)));
-      vr[e] = dR * w + kr[e]; vc[e] = dC * w + kc[e];
-    }
-    for (int qp = 0; qp < geo.npc; ++qp) {
-      __syncthreads();
-      {
-        const int l = qp * 64 + slot;
-        const int qrr = l / w, qcc = l % w;
-        const int r = QR * w + qrr, c = QC * w + qcc;
-        const bool qv = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
-        float x[HH], y[HH];
-#pragma unroll
-        for (int i = 0; i < HH; ++i) { x[i] = 0.f; y[i] = 0.f; }
-        if (qv) {
-          const long long tq = (long long)r * geo.ny + c;
-          load_seg<T, HH>(row_ptr<T>(q, b, h, tq), half * HH, D, x);
-          load_seg<T, HH>(row_ptr<T>(d_o, b, h, tq), half * HH, D, y);
-          if (half == 0) { lse_s[slot] = lse[bh * geo.Nloc + tq]; del_s[slot] = delta[bh * geo.Nloc + tq]; }
-        }
-        stage_half_row<T, HD>(Qs, Qt, x, slot, half);
-        stage_half_row<T, HD>(Gs, Gt, y, slot, half);
-        if (half == 0) { qrs[slot] = (short)qrr; qcs[slot] = (short)qcc; qfl[slot] = (unsigned char)qv; }
+  const int npieces = visit_list(geo, KR, KC, -1, vl) * geo.npc;
+  const int epi = query_epilogue(geo);
+  for (int qp = 0; qp < npieces; ++qp) {
+    __syncthreads();
+    {
+      const int vi = qp / geo.npc, l = (qp - vi * geo.npc) * 64 + slot;
+      bool qv = false;
+      long long tq = 0;
+      int qa = 0, qb = 0, cut = 0;
+      if (l < geo.w2) {
+        const int qrr = l / w, qcc = l - qrr * w;
+        const Visit vq = vl[vi];
+        const int r = vq.r * w + qrr, c = vq.c * w + qcc;
+        qv = (r < geo.nx) && (c < geo.ny);
+        tq = (long long)r * geo.ny + c;
+        qa = qrr - vq.dR * w; qb = qcc - vq.dC * w; cut = vq.cut;
       }
-      sm90::fence_proxy_async();
-      __syncthreads();
-      float s[32], dp[32];
-      sm90::wg_fence();
+      float x[HH], y[HH];
 #pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) W64::ss(s, sm90::desc(Ks, HD, kk), sm90::desc(Qs, HD, kk), kk > 0);
-#pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) W64::ss(dp, sm90::desc(Vs, HD, kk), sm90::desc(Gs, HD, kk), kk > 0);
-      sm90::wg_commit();
-      sm90::wg_wait0();
-      sm90::reg_fence(s);
-      sm90::reg_fence(dp);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int e = (i >> 1) & 1, j = acc_col(i);
-        float p = 0.f, ds = 0.f;
-        if (qfl[j] && kvis[e]) {
-          const int dr = qrs[j] - vr[e], dc = qcs[j] - vc[e];
-          if (!(geo.exact == 1 && (abs(dr) > w || abs(dc) > w))) {
-            const float bias = geo.has_bias ? tab[(dr + 2 * w - 1) * tw + dc + 2 * w - 1] : 0.f;
-            p = __expf(fmaf(geo.scale, s[i], bias) - lse_s[j]);
-            ds = p * (dp[i] - del_s[j]);
-          }
-        }
-        s[i] = p;
-        dp[i] = ds;
+      for (int i = 0; i < HH; ++i) { x[i] = 0.f; y[i] = 0.f; }
+      if (qv) {
+        load_seg<T, HH>(row_ptr<T>(q, b, h, tq), half * HH, D, x);
+        load_seg<T, HH>(row_ptr<T>(d_o, b, h, tq), half * HH, D, y);
       }
-      uint32_t ap[4][4], ad[4][4];
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) { to_a_frag<T>(s, kk, ap[kk]); to_a_frag<T>(dp, kk, ad[kk]); }
-      sm90::wg_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) WHD::rs(dvacc, ap[kk], sm90::desc(Gt, 64, kk), 1);
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) WHD::rs(dkacc, ad[kk], sm90::desc(Qt, 64, kk), 1);
-      sm90::wg_commit();
-      sm90::wg_wait0();
-      sm90::reg_fence(dvacc);
-      sm90::reg_fence(dkacc);
+      stage_half_row<T, HD>(Qs, Qt, x, slot, half);
+      stage_half_row<T, HD>(Gs, Gt, y, slot, half);
+      if (half == 0) {
+        qcol.lse[slot] = qv ? lse[bh * geo.Nloc + tq] : INFINITY;
+        qcol.del[slot] = qv ? delta[bh * geo.Nloc + tq] : 0.f;
+        qcol.tix[slot] = qa * tw + qb;
+        qcol.qr[slot] = (short)qa; qcol.qc[slot] = (short)qb;
+        qcol.cut[slot] = (unsigned char)cut;
+      }
     }
+    sm90::fence_proxy_async();
+    __syncthreads();
+    float s[32], dp[32];
+    sm90::wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk) W64::ss(s, sm90::desc(Ks, HD, kk), sm90::desc(Qs, HD, kk), kk > 0);
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk) W64::ss(dp, sm90::desc(Vs, HD, kk), sm90::desc(Gs, HD, kk), kk > 0);
+    sm90::wg_commit();
+    sm90::wg_wait0();
+    sm90::reg_fence(s);
+    sm90::reg_fence(dp);
+    switch (epi) {   // CTA-uniform
+      case 0: dkv_probs<false, 0>(s, dp, geo, qcol, tab, krow); break;
+      case 1: dkv_probs<false, 1>(s, dp, geo, qcol, tab, krow); break;
+      case 2: dkv_probs<false, 2>(s, dp, geo, qcol, tab, krow); break;
+      case 3: dkv_probs<true, 0>(s, dp, geo, qcol, tab, krow); break;
+      case 4: dkv_probs<true, 1>(s, dp, geo, qcol, tab, krow); break;
+      default: dkv_probs<true, 2>(s, dp, geo, qcol, tab, krow); break;
+    }
+    uint32_t ap[4][4], ad[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) { to_a_frag<T>(s, kk, ap[kk]); to_a_frag<T>(dp, kk, ad[kk]); }
+    sm90::wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) WHD::rs(dvacc, ap[kk], sm90::desc(Gt, 64, kk), 1);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) WHD::rs(dkacc, ad[kk], sm90::desc(Qt, 64, kk), 1);
+    sm90::wg_commit();
+    sm90::wg_wait0();
+    sm90::reg_fence(dvacc);
+    sm90::reg_fence(dkacc);
   }
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
-    if (!kreal[e]) continue;
-    const long long tokk = geo.g + (long long)(KR * w + kr[e]) * geo.ny + (KC * w + kc[e]);
+    if (!krow.real[e]) continue;
+    const long long tokk = geo.g + (long long)(KR * w + krow.kr[e]) * geo.ny + (KC * w + krow.kc[e]);
     store_rows<TO, HD>(dkacc, e, row_ptr_w<TO>(dk, b, h, tokk), D, geo.scale);
     store_rows<TO, HD>(dvacc, e, row_ptr_w<TO>(dv, b, h, tokk), D, 1.f);
   }
