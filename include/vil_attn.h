@@ -47,7 +47,7 @@
 extern "C" {
 #endif
 
-#define VIL_ATTN_ABI_VERSION 2
+#define VIL_ATTN_ABI_VERSION 3
 
 /* element type of q/k/v/o and their gradients (arithmetic is always fp32-accumulated) */
 enum { VIL_F32 = 0, VIL_BF16 = 1, VIL_F16 = 2 };
@@ -128,6 +128,23 @@ typedef struct VilAttnParams {
 
   void*   workspace;       /* device scratch, >= vil_attn_workspace_bytes(), 256-byte aligned */
   int64_t workspace_bytes;
+
+  /* ---- attention dropout (nn.Dropout on the softmax probabilities, longformer2d.py:186, 224); ABI v3 ----
+     0 <= dropout_p < 1 (else VIL_E_BADARG); 0 runs exactly the kernels without dropout.  The backward must be given the
+     forward's p, seed and offset: the mask is recomputed, never stored.  Mask of one element:
+       stream 0, local query rows: row = local token i in [0, nx*ny); col = the column of the reference's attn1:
+                 t for global key t < nglo, nglo + oi*w*w + lk for key lk of the chunk at offset index oi (oi indexes the
+                 reference's block order: 9 blocks for mode 0, [own, neighbour] for mode > 0, own only for mode -1)
+       stream 1, global query rows: row = a in [0, nglo); col = key token j in [0, N)
+       x = Philox4x32-10(key = (seed & 0xffffffff, seed >> 32),
+                         counter = (col >> 2, row, 2*(b*H + h) + stream, (uint32_t)dropout_offset)),  u = x[col & 3]
+       kept iff u >= min(floor(p * 2^32), 2^32 - 1) (computed in double); kept probabilities are scaled by 1.0f/(1.0f - p).
+     A (query, key) pair the reference visits through two offsets is two columns with two draws.  lse / lse_g stay the
+     undropped softmax's. */
+  float    dropout_p;
+  uint32_t reserved2;
+  uint64_t dropout_seed;
+  uint64_t dropout_offset;
 } VilAttnParams;
 
 /* ABI / diagnostics */

@@ -121,17 +121,23 @@ class B200Long2DSCSelfAttention(nn.Module):
         if not x.is_cuda:
             raise RuntimeError("B200Long2DSCSelfAttention only runs on a CUDA (sm_90a) device; there is no CPU "
                                "fallback (use the reference module / oracle for CPU parity checks)")
-        if self.attn_drop.p > 0 and self.training:
-            raise NotImplementedError("attention dropout > 0 is not supported by the fused kernel "
-                                      "(the reference never enables it: build_model does not set attn_drop_rate)")
         if self.only_glo:
             return self._forward_only_glo(x, nx, ny)
         mode = self._pick_mode()
+        drop = self.attn_drop.p if self.training else 0.0
+        if drop >= 1.0:
+            # nn.Dropout(1) zeroes every probability: the attention output is exactly 0 and only proj's bias is left
+            out = x.new_zeros(B, N, C)
+            if defer_proj_bias:
+                return F.linear(out, self.proj.weight), self.proj.bias
+            if g >= 1 and not self.sharew:
+                return self.proj_drop(torch.cat((self.proj_global(out[:, :g]), self.proj(out[:, g:])), dim=1))
+            return self.proj_drop(self.proj(out))
         table = self.local_relative_position_bias_table if self.rpe else None
         g2l = self.g2l_relative_position_bias if (self.rpe and g >= 1) else None
         g2g = self.g2g_relative_position_bias if (self.rpe and g >= 1) else None
         kw = dict(num_heads=H, nx=nx, ny=ny, w=self.attention_window, nglo=g, exact=self.exact, mode=mode,
-                  scale=self.scale, impl=self.impl)
+                  scale=self.scale, impl=self.impl, dropout_p=drop)
         if g >= 1 and self.sharew:
             # one GEMM for local + global queries, the kv GEMM is not recomputed (cf. longformer2d.py:211)
             out = vil_attention(self._lin(self.query, x), self._lin(self.kv, x), None, None, table, g2l, g2g, **kw)
@@ -157,7 +163,7 @@ class B200Long2DSCSelfAttention(nn.Module):
         q = self.scale * self.query(x[:, g:]).reshape(B, N - g, H, M).transpose(1, 2)
         kv = self.kv(x).reshape(B, N, 2, H, M).permute(2, 0, 3, 1, 4)
         k, v = kv[0], kv[1]
-        a1 = (q @ k[:, :, :g].transpose(-2, -1)).softmax(dim=-1)
+        a1 = self.attn_drop((q @ k[:, :, :g].transpose(-2, -1)).softmax(dim=-1))
         x1 = self.proj((a1 @ v[:, :, :g]).transpose(1, 2).reshape(B, N - g, C))
         qg = self.scale * self.query_global(x[:, :g]).reshape(B, g, H, M).transpose(1, 2)
         kvg = self.kv_global(x).reshape(B, N, 2, H, M).permute(2, 0, 3, 1, 4)
@@ -165,7 +171,7 @@ class B200Long2DSCSelfAttention(nn.Module):
         if self.rpe:
             a0 = a0 + torch.cat([self.g2g_relative_position_bias,
                                  self.g2l_relative_position_bias[0].unsqueeze(-1).expand(-1, -1, N - g)], dim=-1)
-        x0 = self.proj_global((a0.softmax(dim=-1) @ kvg[1]).transpose(1, 2).reshape(B, g, C))
+        x0 = self.proj_global((self.attn_drop(a0.softmax(dim=-1)) @ kvg[1]).transpose(1, 2).reshape(B, g, C))
         return self.proj_drop(torch.cat((x0, x1), dim=1))
 
     @staticmethod

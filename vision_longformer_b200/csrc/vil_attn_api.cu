@@ -3,6 +3,7 @@
 // longformer2d.py:22,45-46,111 and slidingchunk_2d.py:331-343), geometry set-up, kernel
 // family selection and launches on the caller's stream.  No allocation, no host sync.
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -85,6 +86,15 @@ int make_geo(const VilAttnParams* p, vil::Geo* g) {
   // the table, so g2l / g2g without a table would be applied by some kernels and ignored by others
   if (!g->has_bias && (p->g2l != nullptr || p->g2g != nullptr))
     return fail(VIL_E_BADARG, "g2l / g2g given without bias_table (rpe parameters come together)");
+  if (!(p->dropout_p >= 0.f && p->dropout_p < 1.f))   // also rejects NaN
+    return fail(VIL_E_BADARG, "dropout_p must be in [0, 1) (got %g)", (double)p->dropout_p);
+  g->drop_p = p->dropout_p;
+  g->drop_scale = 1.0f / (1.0f - p->dropout_p);
+  const double t = std::floor((double)p->dropout_p * 4294967296.0);
+  g->drop_thresh = t >= 4294967295.0 ? 0xffffffffu : (uint32_t)t;
+  g->seed_lo = (uint32_t)(p->dropout_seed & 0xffffffffu);
+  g->seed_hi = (uint32_t)(p->dropout_seed >> 32);
+  g->drop_off = (uint32_t)p->dropout_offset;
   return VIL_OK;
 }
 

@@ -22,6 +22,11 @@ struct Geo {
   int offR[9], offC[9]; // (chunk-row, chunk-col) offsets, reference column order
   int has_bias;
   float scale;
+  // attention dropout (VilAttnParams::dropout_*): a column is kept iff its Philox word >= drop_thresh, and kept
+  // probabilities are scaled by drop_scale = 1 / (1 - p).  Read only by the DROP instantiations of the kernels.
+  float drop_p, drop_scale;
+  uint32_t drop_thresh;
+  uint32_t seed_lo, seed_hi, drop_off;
 };
 
 // backward workspace layout (floats): [delta (B*H*Nloc)] [delta_g (B*H*g)]
@@ -96,6 +101,36 @@ __device__ __forceinline__ void store_seg(T* __restrict__ row, int c0, int D, co
 #pragma unroll
   for (int c = 0; c < CNT; ++c)
     if (c0 + c < D) row[c0 + c] = ElemTraits<T>::from_f(r[c]);
+}
+
+// ---------------------------------------------------------------- attention dropout (include/vil_attn.h, "Attention dropout")
+// Philox4x32-10 (Salmon et al., SC'11; the Random123 constants) of counter (c0, c1, c2, drop_off) under key (seed_lo, seed_hi)
+__device__ __forceinline__ uint4 philox(const Geo& g, uint32_t c0, uint32_t c1, uint32_t c2) {
+  uint32_t x0 = c0, x1 = c1, x2 = c2, x3 = g.drop_off, k0 = g.seed_lo, k1 = g.seed_hi;
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t lo0 = 0xD2511F53u * x0, hi0 = __umulhi(0xD2511F53u, x0);
+    const uint32_t lo1 = 0xCD9E8D57u * x2, hi1 = __umulhi(0xCD9E8D57u, x2);
+    x0 = hi1 ^ x1 ^ k0; x1 = lo1; x2 = hi0 ^ x3 ^ k1; x3 = lo0;
+    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+  }
+  return make_uint4(x0, x1, x2, x3);
+}
+__device__ __forceinline__ uint32_t philox_word(const uint4& x, uint32_t w) {
+  return w == 0 ? x.x : w == 1 ? x.y : w == 2 ? x.z : x.w;
+}
+// Keep bit of one element: row / col are the reference's coordinates, sid = 2 (b H + h) + stream (0: local query rows
+// over the columns of attn1, 1: global query rows over the N keys of attn0)
+__device__ __forceinline__ bool drop_keep(const Geo& g, uint32_t row, uint32_t col, uint32_t sid) {
+  return philox_word(philox(g, col >> 2, row, sid), col & 3) >= g.drop_thresh;
+}
+// Keep bits of the adjacent columns col, col + 1 of one row: one Philox call unless col is the last word of its counter
+__device__ __forceinline__ void drop_keep2(const Geo& g, uint32_t row, uint32_t col, uint32_t sid, bool& k0, bool& k1) {
+  const uint4 x = philox(g, col >> 2, row, sid);
+  const uint32_t w = col & 3;
+  k0 = philox_word(x, w) >= g.drop_thresh;
+  const uint32_t u1 = w == 3 ? philox(g, (col >> 2) + 1, row, sid).x : philox_word(x, w + 1);
+  k1 = u1 >= g.drop_thresh;
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

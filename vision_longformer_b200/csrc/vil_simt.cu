@@ -13,6 +13,7 @@ size_t simt_tile_smem(const Geo& g, int HD, bool dkv) {
   size_t bytes = (size_t)(2 * 64 * (HD + 8) + (g.has_bias ? tw * tw : 0)) * sizeof(float);
   if (dkv) bytes += 2 * 64 * sizeof(float);
   bytes += 64 * 2 * sizeof(short) + 64;
+  if (dkv && g.drop_p > 0.f) bytes += 64 * sizeof(int);          // the query token of each column (dropout rows)
   return (bytes + 15) & ~size_t(15);
 }
 
@@ -84,14 +85,17 @@ int global_bwd_t(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_r
   HDM(__half, __half, CALL)
 
 // ------------------------------------------------------------------ SIMT family proper
-template <typename T, int HD>
+template <typename T, int HD, bool DROP>
 int simt_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+  if constexpr (DROP && HD > 64) {   // the backward stops at 64 as well; at 128 the dropout forward would spill
+    return shared_fail(VIL_E_UNSUPPORTED, "attention dropout supports head dim <= 64");
+  } else {
   const size_t sm = simt_tile_smem(g, HD, false);
-  int rc = set_smem(simt_fwd_local<T, HD>, sm);
+  int rc = set_smem(simt_fwd_local<T, HD, DROP>, sm);
   if (rc) return rc;
   const long long blocks = (long long)g.B * g.H * g.mx * g.my * g.npc;
   if (!(p->skip_mask & 2)) {
-    simt_fwd_local<T, HD><<<(unsigned)blocks, 128, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse, p->bias_table,
+    simt_fwd_local<T, HD, DROP><<<(unsigned)blocks, 128, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse, p->bias_table,
                                                              p->g2l);
     count_launch();
   }
@@ -99,9 +103,10 @@ int simt_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
     if ((rc = global_fwd_t<T, HD, T>(p, g, s))) return rc;
   }
   return launch_check("simt forward");
+  }
 }
 
-template <typename T, int HD>
+template <typename T, int HD, bool DROP>
 int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   if constexpr (HD > 64) {
     return shared_fail(VIL_E_UNSUPPORTED, "backward supports head dim <= 64");
@@ -109,16 +114,16 @@ int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
     int rc = (p->skip_mask & 8) ? VIL_OK : delta_t<T, T>(p, g, s);
     if (rc) return rc;
     const size_t sm1 = simt_tile_smem(g, HD, false), sm2 = simt_tile_smem(g, HD, true);
-    if ((rc = set_smem(simt_bwd_dq<T, HD>, sm1))) return rc;
-    if ((rc = set_smem(simt_bwd_dkv<T, HD>, sm2))) return rc;
+    if ((rc = set_smem(simt_bwd_dq<T, HD, DROP>, sm1))) return rc;
+    if ((rc = set_smem(simt_bwd_dkv<T, HD, DROP>, sm2))) return rc;
     const long long blocks = (long long)g.B * g.H * g.mx * g.my * g.npc;
     if (!(p->skip_mask & 2)) {
-      simt_bwd_dq<T, HD><<<(unsigned)blocks, 128, sm1, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse,
+      simt_bwd_dq<T, HD, DROP><<<(unsigned)blocks, 128, sm1, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse,
                                                             ws_delta(p), p->bias_table, p->g2l, p->d_bias_table);
       count_launch();
     }
     if (!(p->skip_mask & 4)) {
-      simt_bwd_dkv<T, HD><<<(unsigned)blocks, 128, sm2, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv),
+      simt_bwd_dkv<T, HD, DROP><<<(unsigned)blocks, 128, sm2, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv),
                                                              p->lse, ws_delta(p), p->bias_table);
       count_launch();
     }
@@ -129,15 +134,20 @@ int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   }
 }
 
+template <typename T, bool DROP>
+int simt_dispatch_hd(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
+  switch (head_bucket(g.D)) {
+    case 8:   return bwd ? simt_backward<T, 8, DROP>(p, g, s) : simt_forward<T, 8, DROP>(p, g, s);
+    case 16:  return bwd ? simt_backward<T, 16, DROP>(p, g, s) : simt_forward<T, 16, DROP>(p, g, s);
+    case 32:  return bwd ? simt_backward<T, 32, DROP>(p, g, s) : simt_forward<T, 32, DROP>(p, g, s);
+    case 64:  return bwd ? simt_backward<T, 64, DROP>(p, g, s) : simt_forward<T, 64, DROP>(p, g, s);
+    default:  return bwd ? simt_backward<T, 128, DROP>(p, g, s) : simt_forward<T, 128, DROP>(p, g, s);
+  }
+}
+
 template <typename T>
 int simt_dispatch(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
-  switch (head_bucket(g.D)) {
-    case 8:   return bwd ? simt_backward<T, 8>(p, g, s) : simt_forward<T, 8>(p, g, s);
-    case 16:  return bwd ? simt_backward<T, 16>(p, g, s) : simt_forward<T, 16>(p, g, s);
-    case 32:  return bwd ? simt_backward<T, 32>(p, g, s) : simt_forward<T, 32>(p, g, s);
-    case 64:  return bwd ? simt_backward<T, 64>(p, g, s) : simt_forward<T, 64>(p, g, s);
-    default:  return bwd ? simt_backward<T, 128>(p, g, s) : simt_forward<T, 128>(p, g, s);
-  }
+  return g.drop_p > 0.f ? simt_dispatch_hd<T, true>(p, g, s, bwd) : simt_dispatch_hd<T, false>(p, g, s, bwd);
 }
 
 }  // namespace

@@ -44,7 +44,7 @@ __device__ __forceinline__ ChunkId decode_block(const Geo& g, int bid) {
 // forward, local queries.  CTA = one 64-query piece of one chunk of one (b,h); thread pair per query,
 // each thread owns half of the head dimension.
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD>
+template <typename T, int HD, bool DROP = false>
 __global__ void __launch_bounds__(128)
 simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
                const float* __restrict__ table, const float* __restrict__ g2l) {
@@ -77,15 +77,18 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
   for (int i = 0; i < HH; ++i) { qh[i] = 0.f; oh[i] = 0.f; }
   if (qvalid) load_seg<T, HH>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), half * HH, D, qh);
   float m = -INFINITY, lsum = 0.f;
+  const uint32_t drow = (uint32_t)(r * geo.ny + c), dsid = 2u * (uint32_t)(b * geo.H + h);   // dropout: row, stream 0
 
   const int ngp = (geo.g + 63) / 64;
   const int npieces = ngp + geo.noffs * geo.npc;
   for (int pi = 0; pi < npieces; ++pi) {
     const bool isg = pi < ngp;
     int dR = 0, dC = 0, KR = 0, KC = 0, kp = 0;
+    int cbase = pi * 64;                  // dropout: attn1 column of the piece's slot 0
     if (!isg) {
       const int oi = (pi - ngp) / geo.npc;
       kp = (pi - ngp) % geo.npc;
+      if (DROP) cbase = geo.g + oi * geo.w2 + kp * 64;
       dR = geo.offR[oi]; dC = geo.offC[oi];
       KR = R + dR; KC = C + dC;
       if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
@@ -145,23 +148,39 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
       if (ok) {
         const float s = fmaf(geo.scale, sp, bias);
         const float* vd = Vs + j * HS + TL::off(half);
-        if (s > m) {
-          const float corr = __expf(m - s);
-          lsum = lsum * corr + 1.f;
+        if constexpr (DROP) {            // lsum sums the undropped P; O sums P * keep, scaled by 1 / (1 - p) at the end
+          const float km = drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? 1.f : 0.f;
+          if (s > m) {
+            const float corr = __expf(m - s);
+            lsum = lsum * corr + 1.f;
 #pragma unroll
-          for (int i = 0; i < HH; ++i) oh[i] = fmaf(oh[i], corr, vd[i]);
-          m = s;
+            for (int i = 0; i < HH; ++i) oh[i] = fmaf(oh[i], corr, km * vd[i]);
+            m = s;
+          } else {
+            const float p = __expf(s - m);
+            lsum += p;
+#pragma unroll
+            for (int i = 0; i < HH; ++i) oh[i] = fmaf(p * km, vd[i], oh[i]);
+          }
         } else {
-          const float p = __expf(s - m);
-          lsum += p;
+          if (s > m) {
+            const float corr = __expf(m - s);
+            lsum = lsum * corr + 1.f;
 #pragma unroll
-          for (int i = 0; i < HH; ++i) oh[i] = fmaf(p, vd[i], oh[i]);
+            for (int i = 0; i < HH; ++i) oh[i] = fmaf(oh[i], corr, vd[i]);
+            m = s;
+          } else {
+            const float p = __expf(s - m);
+            lsum += p;
+#pragma unroll
+            for (int i = 0; i < HH; ++i) oh[i] = fmaf(p, vd[i], oh[i]);
+          }
         }
       }
     }
   }
   if (qvalid) {
-    const float inv = lsum > 0.f ? 1.f / lsum : 0.f;
+    const float inv = (lsum > 0.f ? 1.f / lsum : 0.f) * (DROP ? geo.drop_scale : 1.f);
 #pragma unroll
     for (int i = 0; i < HH; ++i) oh[i] *= inv;
     const long long tokq = (long long)r * geo.ny + c;
@@ -199,7 +218,7 @@ __device__ __forceinline__ float dot8(const float (&a)[8], const float (&b)[8]) 
 // forward, global query rows: dense attention of the nglo global queries over all N keys
 // (longformer2d.py:210-227).  CTA = one (b, h, a); 8 warps x (32/LPR) rows per iteration.
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO = T>      // TO: element type of the OUTPUT (fp32 in the parity build)
+template <typename T, int HD, typename TO = T, bool DROP = false>   // TO: element type of the OUTPUT (fp32 in the parity build)
 __global__ void __launch_bounds__(256)
 simt_fwd_global(Geo geo, T4 qg, T4 kg, T4 vg, T4 og, float* __restrict__ lse_g, const float* __restrict__ g2l,
                 const float* __restrict__ g2g) {
@@ -232,8 +251,12 @@ simt_fwd_global(Geo geo, T4 qg, T4 kg, T4 vg, T4 og, float* __restrict__ lse_g, 
     if (mn > -INFINITY) {                        // branch-free online softmax step of this row group
       const float corr = __expf(m - mn), p = __expf(sc - mn);
       lsum = fmaf(lsum, corr, p);
+      float pk = p;                              // dropout: O sums P * keep, lsum the undropped P
+      if constexpr (DROP) {
+        if (!drop_keep(geo, (uint32_t)a, (uint32_t)j, 2u * (uint32_t)(b * geo.H + h) + 1u)) pk = 0.f;
+      }
 #pragma unroll
-      for (int i = 0; i < 8; ++i) oacc[i] = fmaf(oacc[i], corr, p * vv[i]);
+      for (int i = 0; i < 8; ++i) oacc[i] = fmaf(oacc[i], corr, pk * vv[i]);
       m = mn;
     }
   }
@@ -258,7 +281,7 @@ simt_fwd_global(Geo geo, T4 qg, T4 kg, T4 vg, T4 og, float* __restrict__ lse_g, 
       const float s2 = (red_m[x] == -INFINITY) ? 0.f : __expf(red_m[x] - M);
       L += red_l[x] * s2; O += red_o[x][tid] * s2;
     }
-    if (tid < D) row_ptr_w<TO>(og, b, h, a)[tid] = ElemTraits<TO>::from_f(O / L);
+    if (tid < D) row_ptr_w<TO>(og, b, h, a)[tid] = ElemTraits<TO>::from_f(DROP ? O / L * geo.drop_scale : O / L);
     if (tid == 0) lse_g[((long long)b * geo.H + h) * geo.g + a] = M + logf(L);
   }
 }
@@ -300,7 +323,7 @@ __global__ void simt_bwd_delta(Geo geo, T4 o, T4 d_o, T4 og, T4 d_og,
 // ----------------------------------------------------------------------------------------------
 // backward pass 1 (query-stationary): dq, d_bias_table.  Same tiling as simt_fwd_local.
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD>
+template <typename T, int HD, bool DROP = false>
 __global__ void __launch_bounds__(128)
 simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse,
             const float* __restrict__ delta, const float* __restrict__ table,
@@ -339,15 +362,18 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
     lse_i = lse[((long long)b * geo.H + h) * geo.Nloc + tokq];
     del_i = delta[((long long)b * geo.H + h) * geo.Nloc + tokq];
   }
+  const uint32_t drow = (uint32_t)tokq, dsid = 2u * (uint32_t)(b * geo.H + h);   // dropout: row, stream 0
 
   const int ngp = (geo.g + 63) / 64;
   const int npieces = ngp + geo.noffs * geo.npc;
   for (int pi = 0; pi < npieces; ++pi) {
     const bool isg = pi < ngp;
     int dR = 0, dC = 0, KR = 0, KC = 0, kp = 0;
+    int cbase = pi * 64;                  // dropout: attn1 column of the piece's slot 0
     if (!isg) {
       const int oi = (pi - ngp) / geo.npc;
       kp = (pi - ngp) % geo.npc;
+      if (DROP) cbase = geo.g + oi * geo.w2 + kp * 64;
       dR = geo.offR[oi]; dC = geo.offC[oi];
       KR = R + dR; KC = C + dC;
       if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
@@ -391,6 +417,8 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
     for (int j = 0; j < 64; ++j) {
       const int f = kfl[j];
       if (!f) continue;
+      float km = 1.f;                                    // dropout: keep / (1 - p) of the column
+      if constexpr (DROP) km = drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? geo.drop_scale : 0.f;
       const float* kd = Ks + j * HS + TL::off(half);
       const float* vd = Vs + j * HS + TL::off(half);
       float sp = 0.f, dpp = 0.f;
@@ -408,6 +436,7 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
       }
       if (ok) {
         const float p = __expf(fmaf(geo.scale, sp, bias) - lse_i);
+        if constexpr (DROP) dpp *= km;
         const float ds = p * (dpp - del_i);
 #pragma unroll
         for (int i = 0; i < HH; ++i) dqh[i] = fmaf(ds, kd[i], dqh[i]);
@@ -427,7 +456,7 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
 // backward pass 2 (key-stationary): dk, dv of the LOCAL key rows.  CTA = one 64-key piece of one
 // key chunk; it walks the query chunks that visit it (the symmetric image of the offset list).
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD>
+template <typename T, int HD, bool DROP = false>
 __global__ void __launch_bounds__(128)
 simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
              const float* __restrict__ delta, const float* __restrict__ table) {
@@ -444,6 +473,7 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
   short* qrs = reinterpret_cast<short*>(del_s + 64);
   short* qcs = qrs + 64;
   unsigned char* qfl = reinterpret_cast<unsigned char*>(qcs + 64);
+  int* qtok = reinterpret_cast<int*>(qfl + 64);            // DROP only: the query token of each staged column
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, KR = cid.R, KC = cid.C;
@@ -500,6 +530,7 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
 #pragma unroll
         for (int i = 0; i < HH; ++i) { qd[i] = qq[i]; gd[i] = gg[i]; }
         if (half == 0) { qrs[slot] = (short)qr; qcs[slot] = (short)qc; qfl[slot] = (unsigned char)qv; }
+        if (DROP && half == 0) qtok[slot] = r * geo.ny + c;
       }
       __syncthreads();
       for (int i2 = 0; i2 < 64; ++i2) {
@@ -516,10 +547,19 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
         if (geo.exact == 1 && (abs(dr) > w || abs(dc) > w)) ok = false;
         if (ok) {
           const float bias = geo.has_bias ? tab[(dr + 2 * w - 1) * tw + dc + 2 * w - 1] : 0.f;
-          const float p = __expf(fmaf(geo.scale, sp, bias) - lse_s[i2]);
-          const float ds = p * (dpp - del_s[i2]);
+          float p = __expf(fmaf(geo.scale, sp, bias) - lse_s[i2]);
+          if constexpr (DROP) {            // dS = P (dP keep / (1 - p) - delta), dV += P keep / (1 - p) dO
+            const float km = drop_keep(geo, (uint32_t)qtok[i2], (uint32_t)(geo.g + oi * geo.w2 + lk), 2u * (uint32_t)(b * geo.H + h))
+                                 ? geo.drop_scale : 0.f;
+            const float ds = p * (dpp * km - del_s[i2]);
+            p *= km;
 #pragma unroll
-          for (int i = 0; i < HH; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
+            for (int i = 0; i < HH; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
+          } else {
+            const float ds = p * (dpp - del_s[i2]);
+#pragma unroll
+            for (int i = 0; i < HH; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
+          }
         }
       }
     }
@@ -547,7 +587,7 @@ __device__ __forceinline__ float block_sum_256(float v, float* red /*[8]*/) {
 // backward, global KEY columns seen by the local queries: dk[t], dv[t] for t < nglo and d_g2l[1][h][t].
 // CTA = one (b, h, t); row groups stride over the local queries.
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO = T>
+template <typename T, int HD, typename TO = T, bool DROP = false>
 __global__ void __launch_bounds__(256)
 simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
               const float* __restrict__ delta, const float* __restrict__ g2l, float* __restrict__ d_g2l) {
@@ -576,11 +616,22 @@ simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
     load_seg<T, 8>(row_ptr<T>(d_o, b, h, ic), 8 * sub, D, gg);
     const float ls = lse[base_l + ic], dl = delta[base_l + ic];
     const float sp = group_sum<LPR>(dot8(qq, k8)), dpp = group_sum<LPR>(dot8(gg, v8));
-    const float p = valid ? __expf(fmaf(geo.scale, sp, bias) - ls) : 0.f;
-    const float ds = p * (dpp - dl);
-    if (sub == 0) adb += ds;
+    float p = valid ? __expf(fmaf(geo.scale, sp, bias) - ls) : 0.f;
+    float dpk = dpp;
+    if constexpr (DROP) {                          // dS = P (dP keep / (1 - p) - delta), dV += P keep / (1 - p) dO
+      const float km = drop_keep(geo, (uint32_t)ic, (uint32_t)t, 2u * (uint32_t)(b * geo.H + h)) ? geo.drop_scale : 0.f;
+      dpk = dpp * km;
+      const float ds = p * (dpk - dl);
+      if (sub == 0) adb += ds;
+      p *= km;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) { adk[i] = fmaf(ds, qq[i], adk[i]); adv[i] = fmaf(p, gg[i], adv[i]); }
+      for (int i = 0; i < 8; ++i) { adk[i] = fmaf(ds, qq[i], adk[i]); adv[i] = fmaf(p, gg[i], adv[i]); }
+    } else {
+      const float ds = p * (dpk - dl);
+      if (sub == 0) adb += ds;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { adk[i] = fmaf(ds, qq[i], adk[i]); adv[i] = fmaf(p, gg[i], adv[i]); }
+    }
   }
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -603,7 +654,7 @@ simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
 // CTA = one (b, h); row groups stride over the keys.  `accumulate` != 0: add into dkg/dvg (they alias dk/dv,
 // already written by the dK/dV pass and simt_bwd_gcol earlier on the same stream); else overwrite.
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO = T>
+template <typename T, int HD, typename TO = T, bool DROP = false>
 __global__ void __launch_bounds__(256)
 simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
               const float* __restrict__ lse_g, const float* __restrict__ delta_g,
@@ -647,7 +698,10 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
       float bias = bl;
       if (geo.has_bias && jc < geo.g) bias = g2g[((long long)h * geo.g + a) * geo.g + jc];
       const float p = valid ? __expf(fmaf(geo.scale, sp, bias) - lg) : 0.f;
-      const float ds = p * (dpp - dg);
+      float km = 1.f;                              // dropout: dS = P (dP keep / (1 - p) - delta), dV += P keep / (1 - p) dO
+      if constexpr (DROP) km = drop_keep(geo, (uint32_t)a, (uint32_t)jc, 2u * (uint32_t)(b * geo.H + h) + 1u) ? geo.drop_scale : 0.f;
+      const float ds = DROP ? p * (dpp * km - dg) : p * (dpp - dg);
+      const float pv = DROP ? p * km : p;
       if (geo.has_bias && valid && sub == 0) {
         if (j < geo.g) { if (d_g2g) atomicAdd(d_g2g + ((long long)h * geo.g + a) * geo.g + j, ds); }
         else adb += ds;
@@ -657,7 +711,7 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
       for (int i = 0; i < 8; ++i) {
         adq[i] = fmaf(ds, kk[i], adq[i]);
         ok_[i] = fmaf(dss, q8[i], ok_[i]);        // dkg_j += scale * ds * qg_a
-        ov_[i] = fmaf(p, g8[i], ov_[i]);          // dvg_j += p * dOg_a
+        ov_[i] = fmaf(pv, g8[i], ov_[i]);         // dvg_j += p * dOg_a
       }
       if (valid && j < rmw_rows && 8 * sub < D) {
         store_seg<TO, 8>(row_ptr_w<TO>(dkg, b, h, j), 8 * sub, D, ok_);
@@ -685,13 +739,20 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
 template <typename T, int HD, typename TO = T>
 inline void launch_global_fwd_kernels(const Geo& g, T4 qg, T4 kg, T4 vg, T4 og, float* lse_g, const float* g2l,
                                       const float* g2g, cudaStream_t s) {
-  simt_fwd_global<T, HD, TO><<<g.B * g.H * g.g, 256, 0, s>>>(g, qg, kg, vg, og, lse_g, g2l, g2g);
+  if (g.drop_p > 0.f) simt_fwd_global<T, HD, TO, true><<<g.B * g.H * g.g, 256, 0, s>>>(g, qg, kg, vg, og, lse_g, g2l, g2g);
+  else simt_fwd_global<T, HD, TO><<<g.B * g.H * g.g, 256, 0, s>>>(g, qg, kg, vg, og, lse_g, g2l, g2g);
 }
 template <typename T, int HD, typename TO = T>
 inline void launch_global_bwd_kernels(const Geo& g, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, T4 qg, T4 kg, T4 vg, T4 d_og,
                                       T4 dqg, T4 dkg, T4 dvg, const float* lse, const float* delta, const float* lse_g,
                                       const float* delta_g, const float* g2l, const float* g2g, float* d_g2l,
                                       float* d_g2g, int accumulate, int rmw_rows, cudaStream_t s) {
+  if (g.drop_p > 0.f) {
+    simt_bwd_gcol<T, HD, TO, true><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, d_g2l);
+    simt_bwd_grow<T, HD, TO, true><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, d_g2l,
+                                                             d_g2g, accumulate, rmw_rows);
+    return;
+  }
   simt_bwd_gcol<T, HD, TO><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, d_g2l);
   simt_bwd_grow<T, HD, TO><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, d_g2l, d_g2g,
                                                   accumulate, rmw_rows);

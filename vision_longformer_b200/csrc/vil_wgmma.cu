@@ -27,13 +27,13 @@ const char* why_not(const VilAttnParams* p, const Geo& g) {
 
 long long blocks(const Geo& g) { return (long long)g.B * g.H * g.mx * g.my * g.npc; }
 
-template <typename T, int HD, typename TO>
+template <typename T, int HD, typename TO, bool DROP>
 int forward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   int rc;
   if (!(p->skip_mask & 2)) {
     const size_t sm = wg::FwdSmem<HD>::total(table_floats(g));
-    if ((rc = set_smem(wg::wg_fwd_local<T, HD, TO>, sm))) return rc;
-    wg::wg_fwd_local<T, HD, TO><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse,
+    if ((rc = set_smem(wg::wg_fwd_local<T, HD, TO, DROP>, sm))) return rc;
+    wg::wg_fwd_local<T, HD, TO, DROP><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse,
                                                                             p->bias_table, p->g2l);
     count_launch();
     if ((rc = launch_check("wgmma_fwd_local"))) return rc;
@@ -42,7 +42,7 @@ int forward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   return VIL_OK;
 }
 
-template <typename T, int HD, typename TO>
+template <typename T, int HD, typename TO, bool DROP>
 int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   int rc;
   if (!(p->skip_mask & 8) && (rc = simt_delta(p, g, s))) return rc;
@@ -50,16 +50,16 @@ int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   const int tabn = table_floats(g);
   if (!(p->skip_mask & 2)) {
     const size_t sm = wg::DqSmem<HD>::total(tabn);
-    if ((rc = set_smem(wg::wg_bwd_dq<T, HD, TO>, sm))) return rc;
-    wg::wg_bwd_dq<T, HD, TO><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq),
+    if ((rc = set_smem(wg::wg_bwd_dq<T, HD, TO, DROP>, sm))) return rc;
+    wg::wg_bwd_dq<T, HD, TO, DROP><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq),
                                                                          p->lse, delta, p->bias_table, p->g2l, p->d_bias_table);
     count_launch();
     if ((rc = launch_check("wgmma_bwd_dq"))) return rc;
   }
   if (!(p->skip_mask & 4)) {
-    const size_t sm = wg::DkvSmem<HD>::total(tabn);
-    if ((rc = set_smem(wg::wg_bwd_dkv<T, HD, TO>, sm))) return rc;
-    wg::wg_bwd_dkv<T, HD, TO><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk),
+    const size_t sm = wg::DkvSmem<HD>::total(tabn, DROP);
+    if ((rc = set_smem(wg::wg_bwd_dkv<T, HD, TO, DROP>, sm))) return rc;
+    wg::wg_bwd_dkv<T, HD, TO, DROP><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk),
                                                                           t4(p->dv), p->lse, delta, p->bias_table);
     count_launch();
     if ((rc = launch_check("wgmma_bwd_dkv"))) return rc;
@@ -68,13 +68,18 @@ int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   return VIL_OK;
 }
 
+template <typename T, typename TO, bool DROP>
+int dispatch_hd_drop(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
+  switch (head_tile(g.D)) {
+    case 16: return bwd ? backward_t<T, 16, TO, DROP>(p, g, s) : forward_t<T, 16, TO, DROP>(p, g, s);
+    case 32: return bwd ? backward_t<T, 32, TO, DROP>(p, g, s) : forward_t<T, 32, TO, DROP>(p, g, s);
+    default: return bwd ? backward_t<T, 64, TO, DROP>(p, g, s) : forward_t<T, 64, TO, DROP>(p, g, s);
+  }
+}
+
 template <typename T, typename TO>
 int dispatch_hd(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
-  switch (head_tile(g.D)) {
-    case 16: return bwd ? backward_t<T, 16, TO>(p, g, s) : forward_t<T, 16, TO>(p, g, s);
-    case 32: return bwd ? backward_t<T, 32, TO>(p, g, s) : forward_t<T, 32, TO>(p, g, s);
-    default: return bwd ? backward_t<T, 64, TO>(p, g, s) : forward_t<T, 64, TO>(p, g, s);
-  }
+  return g.drop_p > 0.f ? dispatch_hd_drop<T, TO, true>(p, g, s, bwd) : dispatch_hd_drop<T, TO, false>(p, g, s, bwd);
 }
 
 int run(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {

@@ -76,6 +76,32 @@ __device__ __forceinline__ void store_rows(const float (&acc)[HD / 2], int e, TO
   }
 }
 
+// Attention dropout of a key piece (forward, pass 1): x[i] *= mul where the element is kept, else 0.  row[e] = the local
+// token of the thread's row e, cbase = the attn1 column of the piece's slot 0 (the slots of a piece are consecutive
+// columns), sid = 2 (b H + h).
+// The keep bits are drawn in a rolled loop: unrolled, the 16 Philox calls cost the forward spills.
+__device__ __forceinline__ void drop_key_piece(float (&x)[32], const Geo& geo, const uint32_t (&row)[2], int cbase, uint32_t sid,
+                                               float mul) {
+  uint32_t keep = 0;
+#pragma unroll 1
+  for (int i = 0; i < 32; i += 2) {
+    bool k0, k1;
+    drop_keep2(geo, (i & 2) ? row[1] : row[0], (uint32_t)(cbase + acc_col(i)), sid, k0, k1);
+    keep |= ((uint32_t)k0 | ((uint32_t)k1 << 1)) << i;
+  }
+#pragma unroll
+  for (int i = 0; i < 32; ++i) x[i] = (keep >> i) & 1u ? x[i] * mul : 0.f;
+}
+
+// local token of the thread's two tile rows (past the image: any value, those rows are dropped)
+__device__ __forceinline__ void drop_rows(const Geo& geo, int R, int C, int piece, uint32_t (&row)[2]) {
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int l = piece * 64 + acc_row(2 * e);
+    row[e] = (uint32_t)((R * geo.w + l / geo.w) * geo.ny + C * geo.w + l % geo.w);
+  }
+}
+
 // The walk.  A CTA lists the chunks it visits once, in shared memory: chunks outside the image are dropped (wrapped when
 // exact == -1), the rest kept in offset order.  The forward and pass 1 take ceil(g / 64) pieces of global keys, then npc
 // pieces per visited chunk; pass 2 takes npc query pieces per chunk that visits its keys.  Each chunk starts a piece of
@@ -85,6 +111,7 @@ struct Visit {
   int r, c;     // the visited chunk
   int dR, dC;   // its offset (key chunk = query chunk + offset)
   int cut;      // exact == -1: bit 0 / 1 = the query chunk + offset is the last chunk row / column (its padded keys are cut)
+  int oi;       // the offset's index in Geo::offR / offC (the reference's block order; dropout columns)
 };
 
 // sgn = +1: the key chunks seen by query chunk (R, C); sgn = -1: the query chunks that see key chunk (R, C)
@@ -96,10 +123,17 @@ __device__ __forceinline__ int visit_list(const Geo& geo, int R, int C, int sgn,
     if (geo.exact == -1) { r = (r + geo.mx) % geo.mx; c = (c + geo.my) % geo.my; }
     else if (r < 0 || r >= geo.mx || c < 0 || c >= geo.my) continue;
     const int qR = sgn > 0 ? R : r, qC = sgn > 0 ? C : c;
-    if (threadIdx.x == 0) vl[n] = Visit{r, c, dR, dC, (qR + dR == geo.mx - 1) | ((qC + dC == geo.my - 1) << 1)};
+    if (threadIdx.x == 0) vl[n] = Visit{r, c, dR, dC, (qR + dR == geo.mx - 1) | ((qC + dC == geo.my - 1) << 1), oi};
     ++n;
   }
   return n;
+}
+
+// attn1 column of slot 0 of key piece pi (ngp pieces of global keys, then npc per visited chunk)
+__device__ __forceinline__ int drop_col_base(const Geo& geo, const Visit* vl, int ngp, int pi) {
+  if (pi < ngp) return pi * 64;
+  const int vi = (pi - ngp) / geo.npc;
+  return geo.g + vl[vi].oi * geo.w2 + (pi - ngp - vi * geo.npc) * 64;
 }
 
 // Key lk (< w^2) of visited chunk v: the token (-1: a zero row), whether the column takes part at all (the pad-cut rule
@@ -250,14 +284,16 @@ template <int HD> struct DqSmem {
 };
 template <int HD> struct DkvSmem {
   static constexpr size_t tiles = 6 * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + kQueryMeta + 15) & ~size_t(15); }
+  static size_t total(int tabn, bool drop = false) {
+    return (tiles + (size_t)tabn * 4 + kQueryMeta + (drop ? 64 * sizeof(int) : 0) + 15) & ~size_t(15);
+  }
 };
 
 // ----------------------------------------------------------------------------------------------
 // forward, local queries
 // ----------------------------------------------------------------------------------------------
 // held to 5 / 3 CTAs per SM (HD <= 32 / 64): left alone, ptxas spends registers on hoisting the column loads and drops one
-template <typename T, int HD, typename TO>
+template <typename T, int HD, typename TO, bool DROP = false>
 __global__ void __launch_bounds__(kThreads, HD <= 32 ? 5 : 3)
 wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const float* __restrict__ table,
              const float* __restrict__ g2l) {
@@ -350,6 +386,11 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     }
 #pragma unroll
     for (int i = 0; i < HH; ++i) oacc[i] *= corr[(i >> 1) & 1];
+    if constexpr (DROP) {    // lsum keeps the undropped P; P V takes P * keep, 1 / (1 - p) is applied by the final store
+      uint32_t drow[2];
+      drop_rows(geo, R, C, cid.piece, drow);
+      drop_key_piece(s, geo, drow, drop_col_base(geo, vl, ngp, pi), 2u * (uint32_t)(b * geo.H + h), 1.f);
+    }
     uint32_t a[4][4];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) to_a_frag<T>(s, kk, a[kk]);
@@ -367,7 +408,8 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     lsum[e] += __shfl_xor_sync(0xffffffffu, lsum[e], 2);
     if (!qrow.ok[e]) continue;
     const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
-    store_rows<TO, HD>(oacc, e, row_ptr_w<TO>(o, b, h, tokq), D, lsum[e] > 0.f ? 1.f / lsum[e] : 0.f);
+    const float inv = lsum[e] > 0.f ? 1.f / lsum[e] : 0.f;
+    store_rows<TO, HD>(oacc, e, row_ptr_w<TO>(o, b, h, tokq), D, DROP ? inv * geo.drop_scale : inv);
     if ((tid & 3) == 0) lse[((long long)b * geo.H + h) * geo.Nloc + tokq] = m[e] + logf(lsum[e]);
   }
 }
@@ -375,7 +417,7 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
 // ----------------------------------------------------------------------------------------------
 // backward pass 1 (query-stationary): dq and the local-bias-table gradient
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO>
+template <typename T, int HD, typename TO, bool DROP = false>
 __global__ void __launch_bounds__(kThreads)
 wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse, const float* __restrict__ delta,
           const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ d_table) {
@@ -460,6 +502,11 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     sm90::reg_fence(s);
     sm90::reg_fence(dp);
     const int gl = geo.g - pi * 64;
+    if constexpr (DROP) {    // dS = P (dP keep / (1 - p) - delta)
+      uint32_t drow[2];
+      drop_rows(geo, R, C, cid.piece, drow);
+      drop_key_piece(dp, geo, drow, drop_col_base(geo, vl, ngp, pi), 2u * (uint32_t)(b * geo.H + h), geo.drop_scale);
+    }
     switch (epi) {   // CTA-uniform
       case 0: dq_scores<false, false>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
       case 1: dq_scores<false, true>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
@@ -498,6 +545,7 @@ struct QueryCols {
   short* qr;
   short* qc;
   unsigned char* cut;    // Visit::cut of the query's chunk
+  int* tok;              // DROP only: the query's local token (the dropout row)
 };
 // key row of the 64-row tile (0 for rows past the chunk, which are computed and dropped)
 struct KRows {
@@ -515,6 +563,7 @@ __device__ __forceinline__ QueryCols query_cols(float* base, Visit*& vl) {
   qc.qr = reinterpret_cast<short*>(vl + 9);
   qc.qc = qc.qr + 64;
   qc.cut = reinterpret_cast<unsigned char*>(qc.qc + 64);
+  qc.tok = reinterpret_cast<int*>(qc.cut + 64);
   return qc;
 }
 
@@ -540,7 +589,7 @@ __device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const
   }
 }
 
-template <typename T, int HD, typename TO>
+template <typename T, int HD, typename TO, bool DROP = false>
 __global__ void __launch_bounds__(kThreads)
 wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse, const float* __restrict__ delta,
            const float* __restrict__ table) {
@@ -626,6 +675,7 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
         qcol.tix[slot] = qa * tw + qb;
         qcol.qr[slot] = (short)qa; qcol.qc[slot] = (short)qb;
         qcol.cut[slot] = (unsigned char)cut;
+        if (DROP) qcol.tok[slot] = (int)tq;
       }
     }
     sm90::fence_proxy_async();
@@ -640,6 +690,16 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     sm90::wg_wait0();
     sm90::reg_fence(s);
     sm90::reg_fence(dp);
+    uint32_t keep = 0;       // dropout: bit i = element i is kept
+    if constexpr (DROP) {    // dS = P (dP keep / (1 - p) - delta); the A operand of dV is P keep / (1 - p)
+      const int vi = qp / geo.npc;
+      const uint32_t c0 = (uint32_t)(geo.g + vl[vi].oi * geo.w2 + cid.piece * 64), sid = 2u * (uint32_t)(b * geo.H + h);
+#pragma unroll 1
+      for (int i = 0; i < 32; ++i)
+        keep |= (uint32_t)drop_keep(geo, (uint32_t)qcol.tok[acc_col(i)], c0 + (uint32_t)acc_row(i), sid) << i;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) dp[i] = (keep >> i) & 1u ? dp[i] * geo.drop_scale : 0.f;
+    }
     switch (epi) {   // CTA-uniform
       case 0: dkv_probs<false, 0>(s, dp, geo, qcol, tab, krow); break;
       case 1: dkv_probs<false, 1>(s, dp, geo, qcol, tab, krow); break;
@@ -647,6 +707,10 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
       case 3: dkv_probs<true, 0>(s, dp, geo, qcol, tab, krow); break;
       case 4: dkv_probs<true, 1>(s, dp, geo, qcol, tab, krow); break;
       default: dkv_probs<true, 2>(s, dp, geo, qcol, tab, krow); break;
+    }
+    if constexpr (DROP) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = (keep >> i) & 1u ? s[i] * geo.drop_scale : 0.f;
     }
     uint32_t ap[4][4], ad[4][4];
 #pragma unroll

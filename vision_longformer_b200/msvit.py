@@ -174,8 +174,7 @@ class DenseAttention(nn.Module):
         return (self.impl == "vil" and x.is_cuda and self.wx == self.wy and w in (7, 14)
                 and x.shape[1] == self.nglo + w * w and (x.shape[2] // self.num_heads) <= 64
                 and (x.shape[2] // self.num_heads) % 8 == 0 and self.nglo <= 8
-                and (torch.is_autocast_enabled("cuda") or x.dtype in (torch.bfloat16, torch.float16))
-                and not (self.training and self.attn_drop.p > 0))
+                and (torch.is_autocast_enabled("cuda") or x.dtype in (torch.bfloat16, torch.float16)))
 
     def _vil_table(self):
         """(2w-1)^2 Swin table -> the operator's (4w-1)^2 layout (index (dr + 2w-1)(4w-1) + dc + 2w-1); differentiable."""
@@ -200,8 +199,11 @@ class DenseAttention(nn.Module):
                 table = self._vil_table()
                 if self.nglo >= 1:
                     g2l, g2g = self.g2l_relative_position_bias, self.g2g_relative_position_bias
+            drop = self.attn_drop.p if self.training else 0.0
+            if drop >= 1.0:         # nn.Dropout(1): the attention output is exactly 0
+                return proj(x.new_zeros(B, N, C))
             out = vil_dense_attention(self.qkv(x), table, g2l, g2g, num_heads=self.num_heads, nx=self.wx, ny=self.wy,
-                                      nglo=self.nglo, scale=self.scale)
+                                      nglo=self.nglo, scale=self.scale, dropout_p=drop)
             return proj(out)
         if self.impl == "vil":
             raise NotImplementedError("DenseAttention(impl='vil') needs a 7x7 or 14x14 token grid, head dim <= 64 and bf16/fp16 on CUDA")

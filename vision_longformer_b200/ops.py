@@ -48,7 +48,8 @@ def _f32c(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
     return t.detach().to(torch.float32).contiguous()
 
 
-def _base_params(q, k, nx, ny, w, nglo, exact, mode, scale, impl, skip_mask=0, flags=0) -> VilAttnParams:
+def _base_params(q, k, nx, ny, w, nglo, exact, mode, scale, impl, skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0,
+                 dropout_offset=0) -> VilAttnParams:
     if exact not in (0, 1, -1):
         raise ValueError("longsc exact should be in [0,1,-1]!")          # slidingchunk_2d.py:343
     if exact == 1 and mode != 0:
@@ -64,7 +65,26 @@ def _base_params(q, k, nx, ny, w, nglo, exact, mode, scale, impl, skip_mask=0, f
     p.scale = float(scale)
     p.skip_mask = int(skip_mask)
     p.flags = int(flags)
+    p.dropout_p = float(dropout_p)
+    p.dropout_seed, p.dropout_offset = int(dropout_seed), int(dropout_offset)
     return p
+
+
+def _dropout_state(device: torch.device, dropout_p: float):
+    """(seed, offset) of one dropout forward, drawn from the default CUDA generator of `device` the way torch's own
+    Philox-based kernels draw theirs: the generator's seed and its current offset, which is then advanced.  Host-side
+    generator state only (no host-device synchronisation); `torch.manual_seed` reproduces it.  The kernels take the
+    offset in units of 4 (one Philox counter word)."""
+    if dropout_p <= 0.0:
+        return 0, 0
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("vil_attention: attention dropout cannot be captured in a CUDA graph (the mask's seed and offset "
+                           "are drawn on the host at each call)")
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    gen = torch.cuda.default_generators[idx]
+    seed, offset = gen.initial_seed(), gen.get_offset()
+    gen.set_offset(offset + 4)
+    return seed, offset // 4
 
 
 def _workspace(p: VilAttnParams, backward: bool, device) -> torch.Tensor:
@@ -78,15 +98,17 @@ def _workspace(p: VilAttnParams, backward: bool, device) -> torch.Tensor:
 
 
 def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx, ny, w, exact=0, mode=0,
-                              scale=1.0, impl="auto", skip_mask=0, flags=0):
+                              scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0):
     """q:(B,H,Nloc,D) k,v:(B,H,N,D) qg:(B,H,g,D) kg,vg:(B,H,N,D) views; o/og preallocated output views.
     `flags`: VIL_FLAG_* of include/vil_attn.h (F32_OUT = 1: o / og are fp32 tensors - the parity build).
+    `dropout_p` > 0: attention dropout with the mask of (dropout_seed, dropout_offset) (include/vil_attn.h); the
+    backward must be given the same three values.
     Returns (lse (B,H,Nloc) fp32, lse_g (B,H,g) fp32 or None)."""
     _require_cuda(q, "q")
     B, H, Nloc, D = q.shape
     g = k.shape[2] - Nloc
     assert Nloc == nx * ny, "Global dimension does not match!"           # longformer2d.py:111
-    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags)
+    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset)
     lse = torch.empty(B, H, Nloc, dtype=torch.float32, device=q.device)
     lse_g = torch.empty(B, H, g, dtype=torch.float32, device=q.device) if g > 0 else None
     p.q, p.k, p.v, p.o = _t4(q), _t4(k), _t4(v), _t4(o)
@@ -104,11 +126,11 @@ def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx
 
 def vil_attention_raw_backward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, lse, lse_g, d_o, d_og,
                                dq, dk, dv, dqg, dkg, dvg, d_table, d_g2l, d_g2g, *, nx, ny, w, exact=0, mode=0,
-                               scale=1.0, impl="auto", skip_mask=0, flags=0):
+                               scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0):
     _require_cuda(q, "q")
     Nloc = q.shape[2]
     g = k.shape[2] - Nloc
-    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags)
+    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset)
     p.q, p.k, p.v, p.o = _t4(q), _t4(k), _t4(v), _t4(o)
     p.d_o, p.dq, p.dk, p.dv = _t4(d_o), _t4(dq), _t4(dk), _t4(dv)
     if g > 0:
@@ -137,7 +159,7 @@ class _VilAttention(torch.autograd.Function):
     # `vil_attention` (not via cast_inputs, which would also round the fp32 bias tables to bf16).
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda")
-    def forward(ctx, q_all, kv, qg_all, kvg, table, g2l, g2g, H, nx, ny, w, nglo, exact, mode, scale, impl):
+    def forward(ctx, q_all, kv, qg_all, kvg, table, g2l, g2g, H, nx, ny, w, nglo, exact, mode, scale, impl, dropout_p):
         _require_cuda(q_all, "q")
         B = q_all.shape[0]
         C = q_all.shape[2]
@@ -165,10 +187,13 @@ class _VilAttention(torch.autograd.Function):
         out = torch.empty(B, N, C, dtype=q_all.dtype, device=q_all.device)
         o = _heads(out, H)[:, :, g:]
         og = _heads(out, H)[:, :, :g] if g > 0 else None
+        seed, offset = _dropout_state(q_all.device, dropout_p)
         lse, lse_g = vil_attention_raw_forward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, nx=nx, ny=ny, w=w,
-                                               exact=exact, mode=mode, scale=scale, impl=impl)
+                                               exact=exact, mode=mode, scale=scale, impl=impl, dropout_p=dropout_p,
+                                               dropout_seed=seed, dropout_offset=offset)
         ctx.save_for_backward(q_all, kv, qg_all, kvg, table, g2l, g2g, out, lse, lse_g)
         ctx.cfg = (H, nx, ny, w, g, exact, mode, scale, impl, shared)
+        ctx.drop = (dropout_p, seed, offset)
         return out
 
     @staticmethod
@@ -176,6 +201,7 @@ class _VilAttention(torch.autograd.Function):
     def backward(ctx, d_out):
         q_all, kv, qg_all, kvg, table, g2l, g2g, out, lse, lse_g = ctx.saved_tensors
         H, nx, ny, w, g, exact, mode, scale, impl, shared = ctx.cfg
+        dropout_p, seed, offset = ctx.drop
         d_out = d_out.contiguous()
         k, v = _heads(kv, H, 0, 2), _heads(kv, H, 1, 2)
         dq_all = torch.empty_like(q_all, memory_format=torch.contiguous_format)
@@ -206,15 +232,16 @@ class _VilAttention(torch.autograd.Function):
         d_g2g = torch.zeros_like(g2g32) if g2g32 is not None else None
         vil_attention_raw_backward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, lse, lse_g, d_o, d_og,
                                    dq, dk, dv, dqg, dkg, dvg, d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=exact,
-                                   mode=mode, scale=scale, impl=impl)
+                                   mode=mode, scale=scale, impl=impl, dropout_p=dropout_p, dropout_seed=seed,
+                                   dropout_offset=offset)
         cast = lambda d, ref: None if d is None else d.to(ref.dtype)
         return (dq_all, dkv, dqg_all, dkvg, cast(d_tab, table) if table is not None else None,
                 cast(d_g2l, g2l) if g2l is not None else None, cast(d_g2g, g2g) if g2g is not None else None,
-                None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None, None)
 
 
 def vil_attention(q_all, kv, qg_all=None, kvg=None, table=None, g2l=None, g2g=None, *, num_heads, nx, ny, w,
-                  nglo, exact=0, mode=0, scale=1.0, impl="auto"):
+                  nglo, exact=0, mode=0, scale=1.0, impl="auto", dropout_p=0.0):
     """Fused local+global Vision-Longformer attention.
 
     shared weights (sharew):   q_all (B, nglo+nx*ny, C) = query(x);          kv (B, N, 2C) = kv(x)
@@ -225,13 +252,16 @@ def vil_attention(q_all, kv, qg_all=None, kvg=None, table=None, g2l=None, g2g=No
     Under `torch.autocast('cuda')` the activations are cast to the autocast dtype first (the reference's
     `@autocast()`-decorated SlidingChunk2D does the same, slidingchunk_2d.py:203,235), so an fp32 caller gets the
     tensor-core path and bf16/fp16 outputs; the bias tables stay fp32.
+
+    `dropout_p` in [0, 1): attention dropout on the probabilities (the reference's `attn_drop`, longformer2d.py:186, 224).
+    Each call draws a fresh mask from the device's default CUDA generator; the backward reuses it.
     """
     if q_all.is_cuda and torch.is_autocast_enabled("cuda"):
         dt = torch.get_autocast_dtype("cuda")
         cast = lambda t: t if (t is None or t.dtype == dt) else t.to(dt)
         q_all, kv, qg_all, kvg = cast(q_all), cast(kv), cast(qg_all), cast(kvg)
     return _VilAttention.apply(q_all, kv, qg_all, kvg, table, g2l, g2g, num_heads, nx, ny, w, nglo, exact, mode,
-                               float(scale), impl)
+                               float(scale), impl, float(dropout_p))
 
 
 class _VilAttentionPacked(torch.autograd.Function):
@@ -242,7 +272,7 @@ class _VilAttentionPacked(torch.autograd.Function):
 
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda")
-    def forward(ctx, qkv, table, g2l, g2g, H, nx, ny, w, nglo, scale):
+    def forward(ctx, qkv, table, g2l, g2g, H, nx, ny, w, nglo, scale, dropout_p):
         _require_cuda(qkv, "qkv")
         B, N, C3 = qkv.shape
         C, g = C3 // 3, nglo
@@ -256,10 +286,13 @@ class _VilAttentionPacked(torch.autograd.Function):
         out = torch.empty(B, N, C, dtype=qkv.dtype, device=qkv.device)
         o = _heads(out, H)[:, :, g:]
         og = _heads(out, H)[:, :, :g] if g > 0 else None
+        seed, offset = _dropout_state(qkv.device, dropout_p)
         lse, lse_g = vil_attention_raw_forward(q, k, v, qg, k if g > 0 else None, v if g > 0 else None, tab32, g2l32, g2g32, o, og,
-                                               nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale)
+                                               nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale, dropout_p=dropout_p,
+                                               dropout_seed=seed, dropout_offset=offset)
         ctx.save_for_backward(qkv, table, g2l, g2g, out, lse, lse_g)
         ctx.cfg = (H, nx, ny, w, g, scale)
+        ctx.drop = (dropout_p, seed, offset)
         return out
 
     @staticmethod
@@ -267,6 +300,7 @@ class _VilAttentionPacked(torch.autograd.Function):
     def backward(ctx, d_out):
         qkv, table, g2l, g2g, out, lse, lse_g = ctx.saved_tensors
         H, nx, ny, w, g, scale = ctx.cfg
+        dropout_p, seed, offset = ctx.drop
         B, N, C3 = qkv.shape
         C = C3 // 3
         d_out = d_out.contiguous()
@@ -283,15 +317,18 @@ class _VilAttentionPacked(torch.autograd.Function):
         d_g2g = torch.zeros_like(g2g32) if g2g32 is not None else None
         kg, vg, dkg, dvg = (k, v, dk, dv) if g > 0 else (None, None, None, None)
         vil_attention_raw_backward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, lse, lse_g, d_o, d_og, dq, dk, dv, dqg, dkg, dvg,
-                                   d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale)
+                                   d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale, dropout_p=dropout_p,
+                                   dropout_seed=seed, dropout_offset=offset)
         cast = lambda d, ref: None if (d is None or ref is None) else d.to(ref.dtype)
-        return d_qkv, cast(d_tab, table), cast(d_g2l, g2l), cast(d_g2g, g2g), None, None, None, None, None, None
+        return d_qkv, cast(d_tab, table), cast(d_g2l, g2l), cast(d_g2g, g2g), None, None, None, None, None, None, None
 
 
-def vil_dense_attention(qkv, table=None, g2l=None, g2g=None, *, num_heads, nx, ny, nglo, scale):
+def vil_dense_attention(qkv, table=None, g2l=None, g2g=None, *, num_heads, nx, ny, nglo, scale, dropout_p=0.0):
     """Dense attention over nglo + nx*ny tokens (nx == ny == w in {7, 14}: one chunk) with the operator's kernels.
-    `table` must already be in the ((4w-1)^2, H) layout of the sliding-chunk operator (see msvit.DenseAttention)."""
+    `table` must already be in the ((4w-1)^2, H) layout of the sliding-chunk operator (see msvit.DenseAttention).
+    `dropout_p`: attention dropout as in `vil_attention`; the mask is the sliding-chunk operator's at mode 0, where the one
+    chunk is the centre block (offset index 4) of attn1."""
     assert nx == ny, "single-chunk dense attention needs a square token grid"
     if qkv.is_cuda and torch.is_autocast_enabled("cuda"):
         qkv = qkv.to(torch.get_autocast_dtype("cuda"))
-    return _VilAttentionPacked.apply(qkv, table, g2l, g2g, num_heads, nx, ny, nx, nglo, float(scale))
+    return _VilAttentionPacked.apply(qkv, table, g2l, g2g, num_heads, nx, ny, nx, nglo, float(scale), float(dropout_p))
