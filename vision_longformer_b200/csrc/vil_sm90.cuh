@@ -1,6 +1,7 @@
 // sm_90a building blocks of the tensor-core family: warpgroup MMA (wgmma.mma_async) with both operands in shared memory
-// (SS) or the A operand in registers (RS), fp32 accumulate.  Hand-written inline PTX; the shared-memory matrix
-// descriptor follows the PTX ISA "Asynchronous Warpgroup Level Matrix" chapter (no-swizzle, K-major core matrices).
+// (SS) or the A operand in registers (RS), fp32 accumulate, and the cp.async copies that stage the operands.  Hand-written
+// inline PTX; the shared-memory matrix descriptors follow the PTX ISA "Asynchronous Warpgroup Level Matrix" chapter
+// (no-swizzle core matrices).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -11,18 +12,38 @@ namespace sm90 {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // Operand tiles are stored as 8 x 8 core matrices of 16-bit elements (8 rows of 16 contiguous bytes, 128 bytes each),
-// row-group major: element (r, c) of a (rows x K) tile sits at core_off(r, c, K).  K-major for both A and B.
+// row-group major: element (r, c) of a (rows x K) tile sits at core_off(r, c, K).
 __host__ __device__ constexpr int core_off(int r, int c, int K) { return (((r >> 3) * (K >> 3) + (c >> 3)) << 6) + ((r & 7) << 3) + (c & 7); }
 
-// Shared-memory matrix descriptor: start address >> 4 [0,14), leading byte offset >> 4 [16,30) (next core matrix
-// along K), stride byte offset >> 4 [32,46) (next 8-row group), layout type [62,64) = 0 (no swizzle).
-__device__ __forceinline__ uint64_t desc(const void* tile, int K, int k16) {
-  const uint32_t a = smem_u32(tile) + k16 * 256;
-  uint64_t d = (uint64_t)((a >> 4) & 0x3FFF);
-  d |= (uint64_t)(128 >> 4) << 16;
-  d |= (uint64_t)(((K >> 3) * 128) >> 4) << 32;
-  return d;
+// Shared-memory matrix descriptor: start address >> 4 [0,14), leading byte offset >> 4 [16,30), stride byte offset >> 4
+// [32,46), layout type [62,64) = 0 (no swizzle).
+__device__ __forceinline__ uint64_t make_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
+  return (uint64_t)((addr >> 4) & 0x3FFF) | (uint64_t)(lbo >> 4) << 16 | (uint64_t)(sbo >> 4) << 32;
 }
+// K-major operand (A, or the B of an SS product): k16 slice of a (rows x K) tile.  LBO = the next core matrix along K,
+// SBO = the next 8-row group.
+__device__ __forceinline__ uint64_t desc(const void* tile, int K, int k16) {
+  return make_desc(smem_u32(tile) + k16 * 256, 128, (K >> 3) * 128);
+}
+// MN-major B operand (the RS products, imm-trans-b = 1): k16 slice of a (K x N) tile stored as core_off(k, n, N), i.e.
+// the same tile that serves as the K-major B of another product.  Its core matrices are 8 K-rows of 8 contiguous
+// N-elements; LBO = the next 8 K-rows, SBO = the next core matrix along N.
+__device__ __forceinline__ uint64_t desc_mn(const void* tile, int N, int k16) {
+  return make_desc(smem_u32(tile) + k16 * N * 32, N * 16, 128);
+}
+
+// cp.async: global -> shared without a register round trip.  n = 16 copies 16 bytes; n = 0 reads nothing and writes 16
+// zero bytes.  Both addresses are 16-byte aligned.
+__device__ __forceinline__ void cp_async16(void* dst, const void* src, int n) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(n) : "memory");
+}
+__device__ __forceinline__ void cp_async4(void* dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// the thread's copies of all but the newest N committed groups have landed
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -46,7 +67,7 @@ __device__ __forceinline__ void wgmma_ss_bf16_n16(float (&d)[8], uint64_t a, uin
 __device__ __forceinline__ void wgmma_rs_bf16_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
@@ -60,7 +81,7 @@ __device__ __forceinline__ void wgmma_ss_f16_n16(float (&d)[8], uint64_t a, uint
 __device__ __forceinline__ void wgmma_rs_f16_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
@@ -74,7 +95,7 @@ __device__ __forceinline__ void wgmma_ss_bf16_n32(float (&d)[16], uint64_t a, ui
 __device__ __forceinline__ void wgmma_rs_bf16_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
@@ -88,7 +109,7 @@ __device__ __forceinline__ void wgmma_ss_f16_n32(float (&d)[16], uint64_t a, uin
 __device__ __forceinline__ void wgmma_rs_f16_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
@@ -102,7 +123,7 @@ __device__ __forceinline__ void wgmma_ss_bf16_n64(float (&d)[32], uint64_t a, ui
 __device__ __forceinline__ void wgmma_rs_bf16_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
@@ -116,11 +137,12 @@ __device__ __forceinline__ void wgmma_ss_f16_n64(float (&d)[32], uint64_t a, uin
 __device__ __forceinline__ void wgmma_rs_f16_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
 
+// Wg<T, N>::ss reads both operands K-major (desc); Wg<T, N>::rs reads its B operand MN-major (desc_mn).
 template <typename T, int N> struct Wg;
 #define VIL_WG(T, TN, N)                                                                                          \
   template <> struct Wg<T, N> {                                                                                   \

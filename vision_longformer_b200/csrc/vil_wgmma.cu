@@ -18,9 +18,17 @@ int set_smem(K kernel, size_t bytes) {
   return VIL_OK;
 }
 
-const char* why_not(const VilAttnParams* p, const Geo& g) {
+// The kernels stage operand rows with 16-byte cp.async copies: every row of the view must start 16-byte aligned.
+bool rows_aligned16(const VilTensor4& t) {
+  constexpr long long e = 2;   // bf16 / fp16
+  return reinterpret_cast<uintptr_t>(t.ptr) % 16 == 0 && (t.sb * e) % 16 == 0 && (t.sh * e) % 16 == 0 && (t.st * e) % 16 == 0;
+}
+
+const char* why_not(const VilAttnParams* p, const Geo& g, bool bwd) {
   if (p->dtype != VIL_BF16 && p->dtype != VIL_F16) return "dtype is fp32 (wgmma operands are bf16 / fp16)";
   if (g.D > 64) return "head dim > 64";
+  if (g.D % 8 != 0 || !rows_aligned16(p->q) || !rows_aligned16(p->k) || !rows_aligned16(p->v) || (bwd && !rows_aligned16(p->d_o)))
+    return "q / k / v / d_o rows are not 16-byte aligned (D % 8 != 0, or a pointer or b / h / t stride off 16 bytes)";
   if (wg::DkvSmem<64>::total(table_floats(g)) > 227 * 1024) return "bias table does not fit in shared memory";
   return nullptr;
 }
@@ -91,11 +99,11 @@ int run(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
 
 }  // namespace
 
-const char* tc_why_not(const VilAttnParams* p, const Geo& g, bool) {
-  const char* w = why_not(p, g);
+const char* tc_why_not(const VilAttnParams* p, const Geo& g, bool bwd) {
+  const char* w = why_not(p, g, bwd);
   return w ? w : "supported";
 }
-int tc_supported(const VilAttnParams* p, const Geo& g, bool) { return why_not(p, g) == nullptr; }
+int tc_supported(const VilAttnParams* p, const Geo& g, bool bwd) { return why_not(p, g, bwd) == nullptr; }
 int tc_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) { return run(p, g, s, false); }
 int tc_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) { return run(p, g, s, true); }
 

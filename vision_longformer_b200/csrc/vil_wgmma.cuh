@@ -2,8 +2,8 @@
 //
 // Same decomposition and masking rules as the SIMT family (vil_simt.cuh), with every product on the tensor cores:
 // a CTA is one warpgroup (128 threads) owning a 64-row tile; it walks 64-column pieces (the global keys, then the
-// visited chunks piece by piece).  Per piece the operands are staged into shared memory as 8x8 core matrices, with the
-// mask / bias terms of every column, and
+// visited chunks piece by piece).  Per piece the operands are copied (cp.async, a few pieces ahead) into shared memory as
+// 8x8 core matrices in their natural (token, d) layout, with the mask / bias terms of every column, and
 //   forward          S = Q K^T (SS), online softmax in registers, O += P V (RS: P stays in registers)
 //   backward pass 1  S = Q K^T, dP = dO V^T (SS), dS = P (dP - delta), dQ += dS K (RS)         (query-stationary)
 //   backward pass 2  S^T = K Q^T, dP^T = V dO^T (SS), dV += P^T dO, dK += dS^T Q (RS)           (key-stationary)
@@ -11,7 +11,9 @@
 //
 // Accumulator fragment of m64nNk16 (fp32): thread t of warp wp holds, for register i, row 16 wp + (t / 4) + 8 ((i / 2) % 2)
 // and column 8 (i / 4) + 2 (t % 4) + (i % 2).  The A fragment of a k16 slice is the same layout over 16 columns, so an
-// accumulator tile converts to the A operand of the next product without leaving registers.
+// accumulator tile converts to the A operand of the next product without leaving registers.  The B operand of an RS
+// product (V, K, dO, Q: consumed along the token axis) is the same (token, d) tile an SS product reads K-major, read
+// MN-major.
 #pragma once
 #include "vil_common.cuh"
 #include "vil_sm90.cuh"
@@ -36,22 +38,23 @@ __device__ __forceinline__ Cta decode(const Geo& g, int bid) {
 __device__ __forceinline__ int acc_row(int i) { return ((threadIdx.x >> 5) << 4) + ((threadIdx.x & 31) >> 2) + (((i >> 1) & 1) << 3); }
 __device__ __forceinline__ int acc_col(int i) { return ((i >> 2) << 3) + ((threadIdx.x & 3) << 1) + (i & 1); }
 
-// half a row (HD/2 values of tile row `row`) -> (64 x HD) core-matrix tile; optionally also into the transposed (HD x 64) tile
+// Ring of operand stages: piece pi is staged into stage pi % kStages while the pieces before it are multiplied, so the
+// copies of kStages - 1 pieces are in flight behind the MMAs of a round.
+constexpr int kStages = 3;
+
+// The thread's row segment of a (64 x HD) tile: row `row`, columns [half HD / 2, (half + 1) HD / 2), copied 16 bytes at a
+// time from row `tok` of the (b, h) slice `base` (row stride st) straight into the core-matrix layout.  tok < 0 (a phantom
+// row) and 8-column groups at or past D are zero-filled without a read: padding keys / queries keep K = V = 0, which the
+// masks rely on (a NaN in a masked column would survive the fmaf with -inf).  Needs D % 8 == 0 and 16-byte aligned rows.
 template <typename T, int HD>
-__device__ __forceinline__ void stage_half_row(T* tile, T* tile_t, const float (&x)[HD / 2], int row, int half) {
+__device__ __forceinline__ void stage_row(T* tile, const T* base, long long st, long long tok, int row, int half, int D) {
   constexpr int HH = HD / 2;
+  const T* src = base + (tok < 0 ? 0 : tok * st);
 #pragma unroll
   for (int g8 = 0; g8 < HH / 8; ++g8) {
-    uint4 u;
-    u.x = sm90::pack2<T>(x[g8 * 8 + 0], x[g8 * 8 + 1]);
-    u.y = sm90::pack2<T>(x[g8 * 8 + 2], x[g8 * 8 + 3]);
-    u.z = sm90::pack2<T>(x[g8 * 8 + 4], x[g8 * 8 + 5]);
-    u.w = sm90::pack2<T>(x[g8 * 8 + 6], x[g8 * 8 + 7]);
-    *reinterpret_cast<uint4*>(tile + sm90::core_off(row, half * HH + g8 * 8, HD)) = u;
-  }
-  if (tile_t != nullptr) {
-#pragma unroll
-    for (int i = 0; i < HH; ++i) tile_t[sm90::core_off(half * HH + i, row, 64)] = ElemTraits<T>::from_f(x[i]);
+    const int c = half * HH + g8 * 8;
+    const bool in = tok >= 0 && c < D;
+    sm90::cp_async16(tile + sm90::core_off(row, c, HD), in ? src + c : base, in ? 16 : 0);
   }
 }
 
@@ -136,10 +139,25 @@ __device__ __forceinline__ int drop_col_base(const Geo& geo, const Visit* vl, in
   return geo.g + vl[vi].oi * geo.w2 + (pi - ngp - vi * geo.npc) * 64;
 }
 
-// Key lk (< w^2) of visited chunk v: the token (-1: a zero row), whether the column takes part at all (the pad-cut rule
-// folded in), and the key's (row, column) relative to the query chunk's origin -- the rules of simt_fwd_local.
-__device__ __forceinline__ void chunk_key(const Geo& geo, const Visit& v, int lk, long long& tok, bool& ok, int& vr, int& vc) {
-  const int w = geo.w, kr = lk / w, kc = lk - kr * w;
+// The thread's slot in the next chunk piece to stage: slot `slot` of piece pj of visited chunk vi is the chunk's position
+// pj * 64 + slot = (kr, kc) (kr >= w: an empty slot).  One piece further is 64 positions further, so walking the pieces in
+// order needs no division.
+struct SlotWalk {
+  int vi, pj, kr, kc;
+  int r0, c0, dr, dc;   // slot / w, slot % w, 64 / w, 64 % w
+  __device__ __forceinline__ SlotWalk(const Geo& geo, int slot)
+      : vi(0), pj(0), r0(slot / geo.w), c0(slot % geo.w), dr(64 / geo.w), dc(64 % geo.w) { kr = r0; kc = c0; }
+  __device__ __forceinline__ void next(const Geo& geo) {
+    if (++pj == geo.npc) { pj = 0; ++vi; kr = r0; kc = c0; return; }
+    kr += dr; kc += dc;
+    if (kc >= geo.w) { kc -= geo.w; ++kr; }
+  }
+};
+
+// Key (kr, kc) (kr < w) of visited chunk v: the token (-1: a zero row), whether the column takes part at all (the pad-cut
+// rule folded in), and the key's (row, column) relative to the query chunk's origin -- the rules of simt_fwd_local.
+__device__ __forceinline__ void chunk_key(const Geo& geo, const Visit& v, int kr, int kc, long long& tok, bool& ok, int& vr, int& vc) {
+  const int w = geo.w;
   const int ar = v.r * w + kr, ac = v.c * w + kc;
   const bool real = (ar < geo.nx) && (ac < geo.ny);
   if (geo.exact == -1)
@@ -150,22 +168,22 @@ __device__ __forceinline__ void chunk_key(const Geo& geo, const Visit& v, int lk
   vr = v.dR * w + kr; vc = v.dC * w + kc;
 }
 
-// Column slot of key piece pi (ngp pieces of global keys, then npc per visited chunk): gk = the global key (-1 for a
-// local one or an empty slot), then as chunk_key.  Global keys sit at (0, 0), which every query of the chunk sees under
-// the exact window.
-__device__ __forceinline__ void key_slot(const Geo& geo, const Visit* vl, int ngp, int pi, int slot, int& gk, long long& tok,
-                                         bool& ok, int& vr, int& vc) {
+// Column slot of key piece pi (ngp pieces of global keys, then npc per visited chunk, taken in order: the chunk pieces
+// advance `wk`): gk = the global key (-1 for a local one or an empty slot), then as chunk_key.  Global keys sit at (0, 0),
+// which every query of the chunk sees under the exact window.
+__device__ __forceinline__ void key_slot(const Geo& geo, const Visit* vl, int ngp, int pi, int slot, SlotWalk& wk, int& gk,
+                                         long long& tok, bool& ok, int& vr, int& vc) {
   gk = -1; tok = -1; ok = false; vr = 0; vc = 0;
   if (pi < ngp) {
     const int t = pi * 64 + slot;
     if (t < geo.g) { gk = t; tok = t; ok = true; }
     return;
   }
-  const int vi = (pi - ngp) / geo.npc, lk = (pi - ngp - vi * geo.npc) * 64 + slot;
-  if (lk < geo.w2) chunk_key(geo, vl[vi], lk, tok, ok, vr, vc);
+  if (wk.kr < geo.w) chunk_key(geo, vl[wk.vi], wk.kr, wk.kc, tok, ok, vr, vc);
+  wk.next(geo);
 }
 
-// Per-column metadata of a staged key piece, written once per round.  The score of (query row, key column j) is
+// Per-column metadata of a staged key piece, written when the piece is issued.  The score of (query row, key column j) is
 // scale * s + bias[j] (+ tab[row base - tix[j]] with the bias table), -inf where bias[j] = -inf or the exact window
 // |qr - kr[j]|, |qc - kc[j]| <= w fails.
 struct KeyCols {
@@ -261,33 +279,65 @@ __device__ __forceinline__ void dq_scores(float (&s)[32], const float (&dp)[32],
   }
 }
 
-constexpr size_t kKeyMeta = 64 * (4 + 4 + 2 + 2) + 9 * sizeof(Visit);
-constexpr size_t kQueryMeta = 64 * (4 + 4 + 4 + 2 + 2 + 1) + 9 * sizeof(Visit);
+// Shared memory of a CTA: the stationary tiles, kStages stages of two streamed tiles each, kStages sets of per-column
+// metadata, the visit list and the bias table.
+constexpr size_t kKeyCols = 64 * (4 + 4 + 2 + 2);
+constexpr size_t kQueryCols = 64 * (4 + 4 + 4 + 2 + 2 + 1);
+constexpr size_t kVisits = 9 * sizeof(Visit);
+// pass 2 with dropout also stages each query column's token
+__host__ __device__ constexpr size_t query_cols_bytes(bool drop) { return kQueryCols + (drop ? 64 * sizeof(int) : 0); }
 
-__device__ __forceinline__ KeyCols key_cols(float* base, Visit*& vl) {
+__device__ __forceinline__ KeyCols key_cols(unsigned char* meta, int stage) {
   KeyCols kc;
-  kc.bias = base;
+  kc.bias = reinterpret_cast<float*>(meta + stage * kKeyCols);
   kc.tix = reinterpret_cast<int*>(kc.bias + 64);
-  vl = reinterpret_cast<Visit*>(kc.tix + 64);
-  kc.kr = reinterpret_cast<short*>(vl + 9);
+  kc.kr = reinterpret_cast<short*>(kc.tix + 64);
   kc.kc = kc.kr + 64;
   return kc;
 }
 
-template <int HD> struct FwdSmem {
-  static constexpr size_t tiles = 3 * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + kKeyMeta + 15) & ~size_t(15); }
+template <int HD> struct FwdSmem {     // Q; K, V per stage
+  static constexpr size_t tiles = (1 + 2 * kStages) * 64 * HD * 2;
+  static size_t total(int tabn) { return (tiles + kStages * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
 };
-template <int HD> struct DqSmem {
-  static constexpr size_t tiles = 5 * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + (size_t)tabn * 4 + kKeyMeta + 15) & ~size_t(15); }
+template <int HD> struct DqSmem {      // Q, dO; K, V per stage
+  static constexpr size_t tiles = (2 + 2 * kStages) * 64 * HD * 2;
+  static size_t total(int tabn) { return (tiles + kStages * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
 };
-template <int HD> struct DkvSmem {
-  static constexpr size_t tiles = 6 * 64 * HD * 2;
+template <int HD> struct DkvSmem {     // K, V; Q, dO per stage; the key rows' chunk positions
+  static constexpr size_t tiles = (2 + 2 * kStages) * 64 * HD * 2;
   static size_t total(int tabn, bool drop = false) {
-    return (tiles + (size_t)tabn * 4 + kQueryMeta + (drop ? 64 * sizeof(int) : 0) + 15) & ~size_t(15);
+    return (tiles + kStages * query_cols_bytes(drop) + kVisits + 64 * sizeof(int) + (size_t)tabn * 4 + 15) & ~size_t(15);
   }
 };
+
+// Stages key piece pi (K and V rows, the column metadata) into ring stage pi % kStages and commits it as one cp.async
+// group; past the last piece it commits an empty group, so that every round waits on the same group count.
+template <typename T, int HD>
+__device__ __forceinline__ void issue_key_piece(const Geo& geo, int pi, int npieces, int ngp, const Visit* vl, SlotWalk& wk,
+                                                T* ring, unsigned char* meta, const T* kb, long long kst, const T* vb,
+                                                long long vst, int h, const float* __restrict__ g2l) {
+  if (pi < npieces) {
+    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = pi % kStages;
+    int gk, vr, vc;
+    long long tok;
+    bool ok;
+    key_slot(geo, vl, ngp, pi, slot, wk, gk, tok, ok, vr, vc);
+    T* Ks = ring + st * 2 * 64 * HD;
+    stage_row<T, HD>(Ks, kb, kst, tok, slot, half, geo.D);
+    stage_row<T, HD>(Ks + 64 * HD, vb, vst, tok, slot, half, geo.D);
+    if (half == 0) stage_key_cols(geo, key_cols(meta, st), h, g2l, gk, ok, vr, vc);
+  }
+  sm90::cp_async_commit();
+}
+
+// Top of round pi: piece pi has landed in every thread's copies, is visible to the async proxy, and every thread is done
+// with round pi - 1, whose stage the next issue refills.
+__device__ __forceinline__ void ring_wait() {
+  sm90::cp_async_wait<kStages - 2>();
+  sm90::fence_proxy_async();
+  __syncthreads();
+}
 
 // ----------------------------------------------------------------------------------------------
 // forward, local queries
@@ -297,17 +347,16 @@ template <typename T, int HD, typename TO, bool DROP = false>
 __global__ void __launch_bounds__(kThreads, HD <= 32 ? 5 : 3)
 wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const float* __restrict__ table,
              const float* __restrict__ g2l) {
-  constexpr int HH = HD / 2;
+  constexpr int HH = HD / 2, TILE = 64 * HD;
   using W64 = sm90::Wg<T, 64>;
   using WHD = sm90::Wg<T, HD>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* Qs = reinterpret_cast<T*>(smem_raw);
-  T* Ks = Qs + 64 * HD;
-  T* Vt = Ks + 64 * HD;
-  float* tab = reinterpret_cast<float*>(Vt + 64 * HD);
+  T* ring = Qs + TILE;                                            // stage s: K at ring + 2 s TILE, V after it
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages * TILE);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kStages * kKeyCols);
+  float* tab = reinterpret_cast<float*>(vl + 9);
   const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
-  Visit* vl;
-  const KeyCols kcol = key_cols(tab + tabn, vl);
 
   const Cta cid = decode(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
@@ -317,11 +366,8 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   {
     const int l = cid.piece * 64 + slot;
     const int r = R * w + l / w, c = C * w + l % w;
-    float x[HH];
-#pragma unroll
-    for (int i = 0; i < HH; ++i) x[i] = 0.f;
-    if (l < geo.w2 && r < geo.nx && c < geo.ny) load_seg<T, HH>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), half * HH, D, x);
-    stage_half_row<T, HD>(Qs, nullptr, x, slot, half);
+    const bool real = l < geo.w2 && r < geo.nx && c < geo.ny;
+    stage_row<T, HD>(Qs, row_ptr<T>(q, b, h, 0), q.st, real ? (long long)r * geo.ny + c : -1, slot, half, D);
   }
   float m[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
   float oacc[HH];
@@ -330,27 +376,20 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
 
   const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, R, C, 1, vl) * geo.npc;
   const int epi = key_epilogue(geo);
+  const T* kb = row_ptr<T>(k, b, h, 0);
+  const T* vb = row_ptr<T>(v, b, h, 0);
+  SlotWalk wk(geo, slot);
+  __syncthreads();                                                // the visit list
+#pragma unroll
+  for (int p = 0; p < kStages - 1; ++p)                           // the first group also carries Q
+    issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
   for (int pi = 0; pi < npieces; ++pi) {
-    __syncthreads();
-    {
-      int gk, vr, vc;
-      long long tok;
-      bool ok;
-      key_slot(geo, vl, ngp, pi, slot, gk, tok, ok, vr, vc);
-      float kk[HH], vv[HH];
-#pragma unroll
-      for (int i = 0; i < HH; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
-      if (tok >= 0) {
-        load_seg<T, HH>(row_ptr<T>(k, b, h, tok), half * HH, D, kk);
-        load_seg<T, HH>(row_ptr<T>(v, b, h, tok), half * HH, D, vv);
-      }
-      stage_half_row<T, HD>(Ks, nullptr, kk, slot, half);
-#pragma unroll
-      for (int i = 0; i < HH; ++i) Vt[sm90::core_off(half * HH + i, slot, 64)] = ElemTraits<T>::from_f(vv[i]);
-      if (half == 0) stage_key_cols(geo, kcol, h, g2l, gk, ok, vr, vc);
-    }
-    sm90::fence_proxy_async();
-    __syncthreads();
+    ring_wait();
+    issue_key_piece<T, HD>(geo, pi + kStages - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    const int st = pi % kStages;
+    const T* Ks = ring + st * 2 * TILE;
+    const T* Vs = Ks + TILE;
+    const KeyCols kcol = key_cols(meta, st);
     float s[32];
     sm90::wg_fence();
 #pragma unroll
@@ -396,7 +435,7 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     for (int kk = 0; kk < 4; ++kk) to_a_frag<T>(s, kk, a[kk]);
     sm90::wg_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) WHD::rs(oacc, a[kk], sm90::desc(Vt, 64, kk), 1);
+    for (int kk = 0; kk < 4; ++kk) WHD::rs(oacc, a[kk], sm90::desc_mn(Vs, HD, kk), 1);
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(oacc);
@@ -421,19 +460,17 @@ template <typename T, int HD, typename TO, bool DROP = false>
 __global__ void __launch_bounds__(kThreads)
 wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse, const float* __restrict__ delta,
           const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ d_table) {
-  constexpr int HH = HD / 2;
+  constexpr int HH = HD / 2, TILE = 64 * HD;
   using W64 = sm90::Wg<T, 64>;
   using WHD = sm90::Wg<T, HD>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* Qs = reinterpret_cast<T*>(smem_raw);
-  T* Gs = Qs + 64 * HD;
-  T* Ks = Gs + 64 * HD;
-  T* Vs = Ks + 64 * HD;
-  T* Kt = Vs + 64 * HD;
-  float* tab = reinterpret_cast<float*>(Kt + 64 * HD);
+  T* Gs = Qs + TILE;
+  T* ring = Gs + TILE;                                            // stage s: K at ring + 2 s TILE, V after it
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages * TILE);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kStages * kKeyCols);
+  float* tab = reinterpret_cast<float*>(vl + 9);
   const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
-  Visit* vl;
-  const KeyCols kcol = key_cols(tab + tabn, vl);
 
   const Cta cid = decode(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
@@ -444,15 +481,9 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   {
     const int l = cid.piece * 64 + slot;
     const int r = R * w + l / w, c = C * w + l % w;
-    float x[HH], y[HH];
-#pragma unroll
-    for (int i = 0; i < HH; ++i) { x[i] = 0.f; y[i] = 0.f; }
-    if (l < geo.w2 && r < geo.nx && c < geo.ny) {
-      load_seg<T, HH>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), half * HH, D, x);
-      load_seg<T, HH>(row_ptr<T>(d_o, b, h, (long long)r * geo.ny + c), half * HH, D, y);
-    }
-    stage_half_row<T, HD>(Qs, nullptr, x, slot, half);
-    stage_half_row<T, HD>(Gs, nullptr, y, slot, half);
+    const long long tokq = (l < geo.w2 && r < geo.nx && c < geo.ny) ? (long long)r * geo.ny + c : -1;
+    stage_row<T, HD>(Qs, row_ptr<T>(q, b, h, 0), q.st, tokq, slot, half, D);
+    stage_row<T, HD>(Gs, row_ptr<T>(d_o, b, h, 0), d_o.st, tokq, slot, half, D);
   }
   const QRows qrow = query_rows(geo, R, C, cid.piece);
   float lse_r[2], del_r[2];
@@ -471,26 +502,20 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
 
   const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, R, C, 1, vl) * geo.npc;
   const int epi = key_epilogue(geo);
-  for (int pi = 0; pi < npieces; ++pi) {
-    __syncthreads();
-    {
-      int gk, vr, vc;
-      long long tok;
-      bool ok;
-      key_slot(geo, vl, ngp, pi, slot, gk, tok, ok, vr, vc);
-      float kk[HH], vv[HH];
+  const T* kb = row_ptr<T>(k, b, h, 0);
+  const T* vb = row_ptr<T>(v, b, h, 0);
+  SlotWalk wk(geo, slot);
+  __syncthreads();                                                // the visit list
 #pragma unroll
-      for (int i = 0; i < HH; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
-      if (tok >= 0) {
-        load_seg<T, HH>(row_ptr<T>(k, b, h, tok), half * HH, D, kk);
-        load_seg<T, HH>(row_ptr<T>(v, b, h, tok), half * HH, D, vv);
-      }
-      stage_half_row<T, HD>(Ks, Kt, kk, slot, half);
-      stage_half_row<T, HD>(Vs, nullptr, vv, slot, half);
-      if (half == 0) stage_key_cols(geo, kcol, h, g2l, gk, ok, vr, vc);
-    }
-    sm90::fence_proxy_async();
-    __syncthreads();
+  for (int p = 0; p < kStages - 1; ++p)                           // the first group also carries Q and dO
+    issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+  for (int pi = 0; pi < npieces; ++pi) {
+    ring_wait();
+    issue_key_piece<T, HD>(geo, pi + kStages - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    const int st = pi % kStages;
+    const T* Ks = ring + st * 2 * TILE;
+    const T* Vs = Ks + TILE;
+    const KeyCols kcol = key_cols(meta, st);
     float s[32], dp[32];
     sm90::wg_fence();
 #pragma unroll
@@ -518,7 +543,7 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     for (int kk = 0; kk < 4; ++kk) to_a_frag<T>(s, kk, a[kk]);
     sm90::wg_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) WHD::rs(dqacc, a[kk], sm90::desc(Kt, 64, kk), 1);
+    for (int kk = 0; kk < 4; ++kk) WHD::rs(dqacc, a[kk], sm90::desc_mn(Ks, HD, kk), 1);
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(dqacc);
@@ -554,17 +579,81 @@ struct KRows {
   bool real[2];
 };
 
-__device__ __forceinline__ QueryCols query_cols(float* base, Visit*& vl) {
+// Chunk position of tile row `row` of key piece `piece`, packed as kr | kc << 8 | (row lies in the chunk) << 16 (w <= 48);
+// rows past the chunk read (0, 0).  Written once per CTA into shared memory, so that the loop runs no division.
+__device__ __forceinline__ int key_pos(const Geo& geo, int piece, int row) {
+  const int lk = piece * 64 + row;
+  return lk < geo.w2 ? (lk / geo.w) | ((lk % geo.w) << 8) | (1 << 16) : 0;
+}
+
+// The thread's two key rows, from the positions key_pos wrote to kpos[64]
+__device__ __forceinline__ KRows key_rows(const Geo& geo, int KR, int KC, const int* kpos) {
+  KRows k;
+  const int w = geo.w, tw = 4 * w - 1;
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int pos = kpos[acc_row(2 * e)];
+    const bool in = pos >> 16;
+    k.kr[e] = pos & 0xff; k.kc[e] = (pos >> 8) & 0xff;
+    k.real[e] = in && (KR * w + k.kr[e] < geo.nx) && (KC * w + k.kc[e] < geo.ny);
+    k.tb[e] = k.kr[e] * tw + k.kc[e] - (2 * w - 1) * (tw + 1);
+    k.cut[e] = (k.kr[e] >= w - geo.padx) | ((k.kc[e] >= w - geo.pady) << 1);
+  }
+  return k;
+}
+
+// the metadata of ring stage `stage`; `bytes` = query_cols_bytes(DROP) per stage
+__device__ __forceinline__ QueryCols query_cols(unsigned char* meta, int stage, int bytes) {
   QueryCols qc;
-  qc.lse = base;
+  qc.lse = reinterpret_cast<float*>(meta + stage * bytes);
   qc.del = qc.lse + 64;
   qc.tix = reinterpret_cast<int*>(qc.del + 64);
-  vl = reinterpret_cast<Visit*>(qc.tix + 64);
-  qc.qr = reinterpret_cast<short*>(vl + 9);
+  qc.qr = reinterpret_cast<short*>(qc.tix + 64);
   qc.qc = qc.qr + 64;
   qc.cut = reinterpret_cast<unsigned char*>(qc.qc + 64);
   qc.tok = reinterpret_cast<int*>(qc.cut + 64);
   return qc;
+}
+
+// Stages query piece qp (Q and dO rows, the column metadata with lse and delta) into ring stage qp % kStages and commits it
+// as one cp.async group (an empty one past the last piece).  The walk runs over the chunks of vl, npc pieces each.
+template <typename T, int HD, bool DROP>
+__device__ __forceinline__ void issue_query_piece(const Geo& geo, int qp, int npieces, const Visit* vl, SlotWalk& wk, T* ring,
+                                                  unsigned char* meta, const T* qb, long long qst, const T* gb, long long gst,
+                                                  const float* __restrict__ lse, const float* __restrict__ delta) {
+  if (qp < npieces) {
+    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = qp % kStages, w = geo.w;
+    bool qv = false;
+    long long tq = 0;
+    int qa = 0, qb2 = 0, cut = 0;
+    if (wk.kr < w) {
+      const Visit vq = vl[wk.vi];
+      const int r = vq.r * w + wk.kr, c = vq.c * w + wk.kc;
+      qv = (r < geo.nx) && (c < geo.ny);
+      tq = (long long)r * geo.ny + c;
+      qa = wk.kr - vq.dR * w; qb2 = wk.kc - vq.dC * w; cut = vq.cut;
+    }
+    wk.next(geo);
+    T* Qs = ring + st * 2 * 64 * HD;
+    stage_row<T, HD>(Qs, qb, qst, qv ? tq : -1, slot, half, geo.D);
+    stage_row<T, HD>(Qs + 64 * HD, gb, gst, qv ? tq : -1, slot, half, geo.D);
+    if (half == 0) {
+      const QueryCols qcol = query_cols(meta, st, (int)query_cols_bytes(DROP));
+      if (qv) {
+        sm90::cp_async4(qcol.lse + slot, lse + tq);
+        sm90::cp_async4(qcol.del + slot, delta + tq);
+      } else {
+        qcol.lse[slot] = INFINITY;
+        qcol.del[slot] = 0.f;
+      }
+      const int tw = 4 * w - 1;
+      qcol.tix[slot] = qa * tw + qb2;
+      qcol.qr[slot] = (short)qa; qcol.qc[slot] = (short)qb2;
+      qcol.cut[slot] = (unsigned char)cut;
+      if (DROP) qcol.tok[slot] = (int)tq;
+    }
+  }
+  sm90::cp_async_commit();
 }
 
 // Pass 2's per-element forms: RPE adds the bias table, MASK 1 is the exact window (exact == 1), MASK 2 the pad cut of
@@ -589,25 +678,26 @@ __device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const
   }
 }
 
+// held to 4 / 3 CTAs per SM (HD <= 32 / 64) without dropout, 3 / 2 with it: left alone, ptxas takes more registers and
+// fits one less
 template <typename T, int HD, typename TO, bool DROP = false>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, (HD <= 32 ? 4 : 3) - (DROP ? 1 : 0))
 wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse, const float* __restrict__ delta,
            const float* __restrict__ table) {
-  constexpr int HH = HD / 2;
+  constexpr int HH = HD / 2, TILE = 64 * HD;
   using W64 = sm90::Wg<T, 64>;
   using WHD = sm90::Wg<T, HD>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* Ks = reinterpret_cast<T*>(smem_raw);
-  T* Vs = Ks + 64 * HD;
-  T* Qs = Vs + 64 * HD;
-  T* Gs = Qs + 64 * HD;
-  T* Qt = Gs + 64 * HD;
-  T* Gt = Qt + 64 * HD;
-  float* tab = reinterpret_cast<float*>(Gt + 64 * HD);
+  T* Vs = Ks + TILE;
+  T* ring = Vs + TILE;                                            // stage s: Q at ring + 2 s TILE, dO after it
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages * TILE);
+  const int cols = (int)query_cols_bytes(DROP);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kStages * cols);
+  int* kpos = reinterpret_cast<int*>(vl + 9);
+  float* tab = reinterpret_cast<float*>(kpos + 64);
   const int tw = 4 * geo.w - 1;
   const int tabn = geo.has_bias ? tw * tw : 0;
-  Visit* vl;
-  const QueryCols qcol = query_cols(tab + tabn, vl);
 
   const Cta cid = decode(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, KR = cid.R, KC = cid.C;
@@ -618,26 +708,10 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
   {
     const int lk = cid.piece * 64 + slot;
     const int ar = KR * w + lk / w, ac = KC * w + lk % w;
-    float x[HH], y[HH];
-#pragma unroll
-    for (int i = 0; i < HH; ++i) { x[i] = 0.f; y[i] = 0.f; }
-    if (lk < geo.w2 && ar < geo.nx && ac < geo.ny) {
-      const long long tokk = geo.g + (long long)ar * geo.ny + ac;
-      load_seg<T, HH>(row_ptr<T>(k, b, h, tokk), half * HH, D, x);
-      load_seg<T, HH>(row_ptr<T>(v, b, h, tokk), half * HH, D, y);
-    }
-    stage_half_row<T, HD>(Ks, nullptr, x, slot, half);
-    stage_half_row<T, HD>(Vs, nullptr, y, slot, half);
-  }
-  KRows krow;
-#pragma unroll
-  for (int e = 0; e < 2; ++e) {
-    const int lk = cid.piece * 64 + acc_row(2 * e);
-    const bool in = lk < geo.w2;
-    krow.kr[e] = in ? lk / w : 0; krow.kc[e] = in ? lk % w : 0;
-    krow.real[e] = in && (KR * w + krow.kr[e] < geo.nx) && (KC * w + krow.kc[e] < geo.ny);
-    krow.tb[e] = krow.kr[e] * tw + krow.kc[e] - (2 * w - 1) * (tw + 1);
-    krow.cut[e] = (krow.kr[e] >= w - geo.padx) | ((krow.kc[e] >= w - geo.pady) << 1);
+    const long long tokk = (lk < geo.w2 && ar < geo.nx && ac < geo.ny) ? geo.g + (long long)ar * geo.ny + ac : -1;
+    stage_row<T, HD>(Ks, row_ptr<T>(k, b, h, 0), k.st, tokk, slot, half, D);
+    stage_row<T, HD>(Vs, row_ptr<T>(v, b, h, 0), v.st, tokk, slot, half, D);
+    if (half == 0) kpos[slot] = key_pos(geo, cid.piece, slot);
   }
   float dkacc[HH], dvacc[HH];
 #pragma unroll
@@ -645,41 +719,32 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
 
   const int npieces = visit_list(geo, KR, KC, -1, vl) * geo.npc;
   const int epi = query_epilogue(geo);
-  for (int qp = 0; qp < npieces; ++qp) {
-    __syncthreads();
-    {
-      const int vi = qp / geo.npc, l = (qp - vi * geo.npc) * 64 + slot;
-      bool qv = false;
-      long long tq = 0;
-      int qa = 0, qb = 0, cut = 0;
-      if (l < geo.w2) {
-        const int qrr = l / w, qcc = l - qrr * w;
-        const Visit vq = vl[vi];
-        const int r = vq.r * w + qrr, c = vq.c * w + qcc;
-        qv = (r < geo.nx) && (c < geo.ny);
-        tq = (long long)r * geo.ny + c;
-        qa = qrr - vq.dR * w; qb = qcc - vq.dC * w; cut = vq.cut;
-      }
-      float x[HH], y[HH];
+  SlotWalk wk(geo, slot);
+  // the (b, h) slices of q, dO, lse and delta are recomputed at each issue: kept live across the loop, they cost the
+  // dropout kernel at HD 32 a spill
+  __syncthreads();                                                // the visit list, kpos
 #pragma unroll
-      for (int i = 0; i < HH; ++i) { x[i] = 0.f; y[i] = 0.f; }
-      if (qv) {
-        load_seg<T, HH>(row_ptr<T>(q, b, h, tq), half * HH, D, x);
-        load_seg<T, HH>(row_ptr<T>(d_o, b, h, tq), half * HH, D, y);
-      }
-      stage_half_row<T, HD>(Qs, Qt, x, slot, half);
-      stage_half_row<T, HD>(Gs, Gt, y, slot, half);
-      if (half == 0) {
-        qcol.lse[slot] = qv ? lse[bh * geo.Nloc + tq] : INFINITY;
-        qcol.del[slot] = qv ? delta[bh * geo.Nloc + tq] : 0.f;
-        qcol.tix[slot] = qa * tw + qb;
-        qcol.qr[slot] = (short)qa; qcol.qc[slot] = (short)qb;
-        qcol.cut[slot] = (unsigned char)cut;
-        if (DROP) qcol.tok[slot] = (int)tq;
-      }
+  for (int p = 0; p < kStages - 1; ++p)                           // the first group also carries K and V
+    issue_query_piece<T, HD, DROP>(geo, p, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
+                                   row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
+  for (int qp = 0; qp < npieces; ++qp) {
+    ring_wait();
+    issue_query_piece<T, HD, DROP>(geo, qp + kStages - 1, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
+                                   row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
+    const int st = qp % kStages;
+    const T* Qs = ring + st * 2 * TILE;
+    const T* Gs = Qs + TILE;
+    const QueryCols qcol = query_cols(meta, st, cols);
+    // dropout: bit i = element i is kept.  Drawn before the products: the draws need neither, and with s and dp not yet
+    // live the Philox rounds fit 3 CTAs per SM without spilling (HD <= 32).
+    uint32_t keep = 0;
+    if constexpr (DROP) {
+      const int vi = qp / geo.npc;
+      const uint32_t c0 = (uint32_t)(geo.g + vl[vi].oi * geo.w2 + cid.piece * 64), sid = 2u * (uint32_t)(b * geo.H + h);
+#pragma unroll 1
+      for (int i = 0; i < 32; ++i)
+        keep |= (uint32_t)drop_keep(geo, (uint32_t)qcol.tok[acc_col(i)], c0 + (uint32_t)acc_row(i), sid) << i;
     }
-    sm90::fence_proxy_async();
-    __syncthreads();
     float s[32], dp[32];
     sm90::wg_fence();
 #pragma unroll
@@ -690,23 +755,18 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     sm90::wg_wait0();
     sm90::reg_fence(s);
     sm90::reg_fence(dp);
-    uint32_t keep = 0;       // dropout: bit i = element i is kept
     if constexpr (DROP) {    // dS = P (dP keep / (1 - p) - delta); the A operand of dV is P keep / (1 - p)
-      const int vi = qp / geo.npc;
-      const uint32_t c0 = (uint32_t)(geo.g + vl[vi].oi * geo.w2 + cid.piece * 64), sid = 2u * (uint32_t)(b * geo.H + h);
-#pragma unroll 1
-      for (int i = 0; i < 32; ++i)
-        keep |= (uint32_t)drop_keep(geo, (uint32_t)qcol.tok[acc_col(i)], c0 + (uint32_t)acc_row(i), sid) << i;
 #pragma unroll
       for (int i = 0; i < 32; ++i) dp[i] = (keep >> i) & 1u ? dp[i] * geo.drop_scale : 0.f;
     }
+    // the key rows are read from kpos where they are used: kept live across the loop, they cost the HD 32 kernel a spill
     switch (epi) {   // CTA-uniform
-      case 0: dkv_probs<false, 0>(s, dp, geo, qcol, tab, krow); break;
-      case 1: dkv_probs<false, 1>(s, dp, geo, qcol, tab, krow); break;
-      case 2: dkv_probs<false, 2>(s, dp, geo, qcol, tab, krow); break;
-      case 3: dkv_probs<true, 0>(s, dp, geo, qcol, tab, krow); break;
-      case 4: dkv_probs<true, 1>(s, dp, geo, qcol, tab, krow); break;
-      default: dkv_probs<true, 2>(s, dp, geo, qcol, tab, krow); break;
+      case 0: dkv_probs<false, 0>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
+      case 1: dkv_probs<false, 1>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
+      case 2: dkv_probs<false, 2>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
+      case 3: dkv_probs<true, 0>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
+      case 4: dkv_probs<true, 1>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
+      default: dkv_probs<true, 2>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
     }
     if constexpr (DROP) {
 #pragma unroll
@@ -717,14 +777,15 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     for (int kk = 0; kk < 4; ++kk) { to_a_frag<T>(s, kk, ap[kk]); to_a_frag<T>(dp, kk, ad[kk]); }
     sm90::wg_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) WHD::rs(dvacc, ap[kk], sm90::desc(Gt, 64, kk), 1);
+    for (int kk = 0; kk < 4; ++kk) WHD::rs(dvacc, ap[kk], sm90::desc_mn(Gs, HD, kk), 1);
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) WHD::rs(dkacc, ad[kk], sm90::desc(Qt, 64, kk), 1);
+    for (int kk = 0; kk < 4; ++kk) WHD::rs(dkacc, ad[kk], sm90::desc_mn(Qs, HD, kk), 1);
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(dvacc);
     sm90::reg_fence(dkacc);
   }
+  const KRows krow = key_rows(geo, KR, KC, kpos);
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     if (!krow.real[e]) continue;
