@@ -126,7 +126,10 @@ typedef struct VilAttnParams {
   float* d_g2l;            /* fp32 (2,H,nglo), accumulated into, or NULL */
   float* d_g2g;            /* fp32 (H,nglo,nglo), accumulated into, or NULL */
 
-  void*   workspace;       /* device scratch, >= vil_attn_workspace_bytes(), 256-byte aligned */
+  void*   workspace;       /* device scratch, >= vil_attn_workspace_bytes(), 256-byte aligned.  The backward keeps
+                              delta = rowsum(dO * O) of the local and global rows there and, when bias_table != NULL,
+                              the partial sums of the three bias gradients (a bounded set for the table: it does not
+                              grow with B; per image for g2l / g2g) */
   int64_t workspace_bytes;
 
   /* ---- attention dropout (nn.Dropout on the softmax probabilities, longformer2d.py:186, 224); ABI v3 ----
@@ -167,7 +170,11 @@ int vil_attn_wgmma_supported(const VilAttnParams* p);
 /* fused forward: o, og, lse, lse_g.  `stream` is a cudaStream_t. */
 int vil_attn_fwd_sm100(const VilAttnParams* p, void* stream);
 
-/* fused backward: dq, dk, dv, dqg, (dkg, dvg), d_bias_table, d_g2l, d_g2g. */
+/* fused backward: dq, dk, dv, dqg, (dkg, dvg), d_bias_table, d_g2l, d_g2g.
+   Deterministic: for a given build and GPU model, identical inputs give bitwise-identical outputs, including the three
+   bias gradients, however the launches and CTAs are scheduled.  No output is summed with atomics: the bias gradients
+   are reduced from workspace partials in a fixed order (which order is an implementation detail, not part of the ABI)
+   and then added into d_bias_table / d_g2l / d_g2g. */
 int vil_attn_bwd_sm100(const VilAttnParams* p, void* stream);
 
 /*

@@ -9,7 +9,9 @@ parameter / buffer names, so checkpoints (utils/checkpoint.py:32-41,98-108),
 
 The q / kv / proj Linears stay stock PyTorch (north star); everything between
 them is ONE fused CUDA operator (`ops.vil_attention`).  There is no CPU path:
-calling forward on CPU tensors raises.
+calling forward on CPU tensors raises.  Its backward is deterministic, with or
+without the relative-position bias (rpe): identical inputs give bitwise-identical
+gradients, and it runs under torch.use_deterministic_algorithms(True).
 """
 from __future__ import annotations
 

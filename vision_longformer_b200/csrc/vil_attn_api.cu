@@ -2,6 +2,7 @@
 // Host-side only: argument validation (mirroring the reference's asserts / ValueErrors,
 // longformer2d.py:22,45-46,111 and slidingchunk_2d.py:331-343), geometry set-up, kernel
 // family selection and launches on the caller's stream.  No allocation, no host sync.
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
@@ -12,6 +13,8 @@
 #include "vil_layernorm.cuh"
 
 namespace {
+
+constexpr int kSMs = 132;                       // H100 SXM
 
 thread_local char g_err[512] = "";
 thread_local const char* g_last_impl = "none";
@@ -80,6 +83,10 @@ int make_geo(const VilAttnParams* p, vil::Geo* g) {
   }
   g->has_bias = p->bias_table != nullptr;
   g->scale = p->scale;
+  // pass-1 image slices with the bias table: about 8 CTAs per SM in all, several waves at the 2-4 CTAs per SM that the
+  // pass-1 kernels fit, and never more slices than images
+  const long long per_slice = (long long)p->H * g->mx * g->my * g->npc;
+  g->nslice = (int)std::min<long long>(p->B, (8LL * kSMs + per_slice - 1) / per_slice);
   if (g->has_bias && p->nglo > 0 && (p->g2l == nullptr || p->g2g == nullptr))
     return fail(VIL_E_BADARG, "bias_table given but g2l / g2g missing while nglo > 0");
   // the reference creates the three bias parameters together (rpe, longformer2d.py:68-100): every kernel family keys them on
@@ -164,8 +171,6 @@ void note_kernel(const char* name) { g_last_kernel = name; }
 }  // namespace vil
 
 namespace {
-
-constexpr int kSMs = 132;                       // H100 SXM
 
 // backward grid: enough warps to cover HBM latency (up to 8 CTAs x 8 warps per SM), fewer for short streams so the
 // per-warp partial d_gamma / d_beta rows stay small next to the activations

@@ -27,11 +27,24 @@ struct Geo {
   float drop_p, drop_scale;
   uint32_t drop_thresh;
   uint32_t seed_lo, seed_hi, drop_off;
+  // with the bias table: backward pass 1 runs nslice * H * mx * my * npc CTAs, CTA slice s taking the images
+  // s, s + nslice, ...; a function of the geometry and the SM count only, so the table partials do not grow with B
+  int nslice;
 };
 
-// backward workspace layout (floats): [delta (B*H*Nloc)] [delta_g (B*H*g)]
-inline long long ws_off_delta_g(const Geo& g) { return ((long long)g.B * g.H * g.Nloc + 63) & ~63LL; }
-inline long long ws_floats(const Geo& g) { return ws_off_delta_g(g) + (((long long)g.B * g.H * g.g + 63) & ~63LL); }
+// backward workspace layout (floats), each part 64-float aligned:
+//   [delta (B*H*Nloc)] [delta_g (B*H*g)]
+//   with the bias table only: [table partials (nslice*H*mx*my*npc, (4w-1)^2): one row per pass-1 CTA]
+//                             [global-bias partials: d_g2l[1] (B,H,g) | d_g2l[0] (B,H,g) | d_g2g (B,H,g,g)]
+inline long long ws_align(long long n) { return (n + 63) & ~63LL; }
+inline long long ws_off_delta_g(const Geo& g) { return ws_align((long long)g.B * g.H * g.Nloc); }
+inline int table_entries(const Geo& g) { return (4 * g.w - 1) * (4 * g.w - 1); }
+inline long long tab_ctas(const Geo& g) { return (long long)g.nslice * g.H * g.mx * g.my * g.npc; }
+inline long long ws_off_tab(const Geo& g) { return ws_off_delta_g(g) + ws_align((long long)g.B * g.H * g.g); }
+inline long long ws_off_glob(const Geo& g) { return ws_off_tab(g) + (g.has_bias ? ws_align(tab_ctas(g) * table_entries(g)) : 0); }
+inline long long ws_floats(const Geo& g) {
+  return ws_off_glob(g) + (g.has_bias && g.g > 0 ? ws_align((long long)g.B * g.H * g.g * (2 + g.g)) : 0);
+}
 
 struct T4 {             // device view (B,H,T,D), unit stride on D
   char* p;
@@ -131,6 +144,35 @@ __device__ __forceinline__ void drop_keep2(const Geo& g, uint32_t row, uint32_t 
   k0 = philox_word(x, w) >= g.drop_thresh;
   const uint32_t u1 = w == 3 ? philox(g, (col >> 2) + 1, row, sid).x : philox_word(x, w + 1);
   k1 = u1 >= g.drop_thresh;
+}
+
+// ---------------------------------------------------------------- bias-table gradient in a fixed order (backward pass 1)
+// tile[i * ld + j] holds dS of query slot i of query piece qp and key slot j of key piece kp of the chunk at offset
+// (dR, dC); masked pairs, rows past the chunk and empty slots hold 0.  The pair (query qr, qc; key kr, kc) adds to entry
+// (qr - kr - dR w + 2w - 1) (4w - 1) + (qc - kc - dC w + 2w - 1).  The pairs of one entry have one (u, v) = (qr - kr,
+// qc - kc), so its queries form a rectangle, clipped to the two pieces' slot ranges row by row.  The (2w - 1)^2 windows
+// (u, v) are dealt out to the 128 threads; each adds its pairs in ascending query-slot order and then adds that sum to
+// acc[entry], which no other thread touches until the next barrier.  Every CTA thereby sums in one fixed order.
+__device__ __forceinline__ void table_grad_piece(const float* tile, int ld, float* acc, const Geo& geo, int dR, int dC,
+                                                 int qp, int kp) {
+  const int w = geo.w, tw = 4 * w - 1, ww = 2 * w - 1;
+  const int q0 = qp * 64, k0 = kp * 64;
+  for (int x = threadIdx.x; x < ww * ww; x += 128) {
+    const int u = x / ww - (w - 1), v = x % ww - (w - 1);
+    const int c_lo = max(0, v), c_hi = min(w - 1, w - 1 + v);
+    float sum = 0.f;
+    bool any = false;
+    for (int qr = max(0, u); qr <= min(w - 1, w - 1 + u); ++qr) {
+      const int kr = qr - u;
+      // query slot qr w + qc in [q0, q0 + 64), key slot kr w + qc - v in [k0, k0 + 64)
+      const int lo = max(c_lo, max(q0 - qr * w, k0 - kr * w + v));
+      const int hi = min(c_hi, min(q0 + 63 - qr * w, k0 + 63 - kr * w + v));
+      const int base = (qr * w - q0) * ld + (kr * w - v - k0);
+      for (int qc = lo; qc <= hi; ++qc) sum += tile[base + qc * (ld + 1)];
+      any |= lo <= hi;
+    }
+    if (any) acc[(u - dR * w + 2 * w - 1) * tw + (v - dC * w + 2 * w - 1)] += sum;
+  }
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

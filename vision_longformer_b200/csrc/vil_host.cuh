@@ -25,12 +25,18 @@ inline T4 t4(const VilTensor4& t) { T4 r; r.p = static_cast<char*>(t.ptr); r.sb 
 // flags of VilAttnParams
 inline bool out_f32(const VilAttnParams* p) { return (p->flags & VIL_FLAG_F32_OUT) != 0; }
 
+// the backward workspace at float offset `off` (vil_common.cuh: ws_off_*)
+inline float* ws_at(const VilAttnParams* p, long long off) { return static_cast<float*>(p->workspace) + off; }
+
 // ---- vil_simt.cu: the CUDA-core family and the small global-token kernels both families share
 int simt_run(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd);
 int simt_global_fwd(const VilAttnParams* p, const Geo& g, cudaStream_t s);                 // og, lse_g
 int simt_delta(const VilAttnParams* p, const Geo& g, cudaStream_t s);                      // delta, delta_g -> workspace
 // global key columns + global query rows; rmw_rows: keys whose dk / dv rows simt_bwd_grow still updates
 int simt_global_bwd(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_rows);
+// with the bias table: sums the partials pass 1 and the global-token kernels left in the workspace, in a fixed order, into
+// d_bias_table, d_g2l, d_g2g (one launch; none without the table)
+int simt_bias_reduce(const VilAttnParams* p, const Geo& g, cudaStream_t s);
 
 // ---- vil_wgmma.cu: the tensor-core (wgmma) family
 const char* tc_why_not(const VilAttnParams* p, const Geo& g, bool bwd);

@@ -53,7 +53,7 @@ int global_bwd_t(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_r
   launch_global_bwd_kernels<T, HD, TO>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv), t4(p->qg), t4(p->kg),
                                        t4(p->vg), t4(p->d_og), t4(p->dqg), t4(shared ? p->dk : p->dkg),
                                        t4(shared ? p->dv : p->dvg), p->lse, ws_delta(p), p->lse_g, ws_delta_g(p, g), p->g2l,
-                                       p->g2g, p->d_g2l, p->d_g2g, shared ? 1 : 0, rmw_rows, s);
+                                       p->g2g, g.has_bias ? ws_at(p, ws_off_glob(g)) : nullptr, shared ? 1 : 0, rmw_rows, s);
   count_launch();
   count_launch();
   return launch_check("simt_bwd_gcol / simt_bwd_grow");
@@ -106,6 +106,20 @@ int simt_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   }
 }
 
+// backward pass 1; TAB (the bias table): nslice image slices per (head, chunk, piece), table partials into the workspace
+template <typename T, int HD, bool DROP, bool TAB>
+int simt_dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+  const size_t sm = simt_tile_smem(g, HD, false) + (TAB ? simt_ds_tile_bytes() : 0);
+  int rc = set_smem(simt_bwd_dq<T, HD, DROP, TAB>, sm);
+  if (rc) return rc;
+  const long long ctas = TAB ? tab_ctas(g) : (long long)g.B * g.H * g.mx * g.my * g.npc;
+  simt_bwd_dq<T, HD, DROP, TAB><<<(unsigned)ctas, 128, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse,
+                                                                ws_delta(p), p->bias_table, p->g2l,
+                                                                TAB ? ws_at(p, ws_off_tab(g)) : nullptr);
+  count_launch();
+  return VIL_OK;
+}
+
 template <typename T, int HD, bool DROP>
 int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   if constexpr (HD > 64) {
@@ -113,14 +127,11 @@ int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   } else {
     int rc = (p->skip_mask & 8) ? VIL_OK : delta_t<T, T>(p, g, s);
     if (rc) return rc;
-    const size_t sm1 = simt_tile_smem(g, HD, false), sm2 = simt_tile_smem(g, HD, true);
-    if ((rc = set_smem(simt_bwd_dq<T, HD, DROP>, sm1))) return rc;
+    const size_t sm2 = simt_tile_smem(g, HD, true);
     if ((rc = set_smem(simt_bwd_dkv<T, HD, DROP>, sm2))) return rc;
     const long long blocks = (long long)g.B * g.H * g.mx * g.my * g.npc;
     if (!(p->skip_mask & 2)) {
-      simt_bwd_dq<T, HD, DROP><<<(unsigned)blocks, 128, sm1, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse,
-                                                            ws_delta(p), p->bias_table, p->g2l, p->d_bias_table);
-      count_launch();
+      if ((rc = g.has_bias ? simt_dq_pass<T, HD, DROP, true>(p, g, s) : simt_dq_pass<T, HD, DROP, false>(p, g, s))) return rc;
     }
     if (!(p->skip_mask & 4)) {
       simt_bwd_dkv<T, HD, DROP><<<(unsigned)blocks, 128, sm2, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv),
@@ -130,7 +141,8 @@ int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
     if (g.g > 0 && !(p->skip_mask & 1)) {
       if ((rc = global_bwd_t<T, HD, T>(p, g, s, g.N))) return rc;
     }
-    return launch_check("simt backward");
+    if ((rc = launch_check("simt backward"))) return rc;
+    return simt_bias_reduce(p, g, s);
   }
 }
 
@@ -172,6 +184,18 @@ int simt_delta(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   if (p->dtype == VIL_F32) return delta_t<float, float>(p, g, s);
   if (p->dtype == VIL_BF16) return out_f32(p) ? delta_t<__nv_bfloat16, float>(p, g, s) : delta_t<__nv_bfloat16, __nv_bfloat16>(p, g, s);
   return out_f32(p) ? delta_t<__half, float>(p, g, s) : delta_t<__half, __half>(p, g, s);
+}
+
+int simt_bias_reduce(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+  if (!g.has_bias) return VIL_OK;
+  // only the partials of kernels that ran (skip_mask) are summed
+  const long long ntab = (p->skip_mask & 2) ? 0 : (long long)table_entries(g) * g.H;
+  const long long nglob = (g.g == 0 || (p->skip_mask & 1)) ? 0 : (long long)g.H * g.g * (2 + g.g);
+  if (ntab + nglob == 0) return VIL_OK;
+  simt_bwd_bias_reduce<<<(unsigned)((ntab + nglob + 255) / 256), 256, 0, s>>>(
+      g, ws_at(p, ws_off_tab(g)), ws_at(p, ws_off_glob(g)), p->d_bias_table, p->d_g2l, p->d_g2g, (int)ntab, (int)nglob);
+  count_launch();
+  return launch_check("simt_bwd_bias_reduce");
 }
 
 int simt_global_bwd(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_rows) {

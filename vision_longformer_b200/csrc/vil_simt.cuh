@@ -321,13 +321,18 @@ __global__ void simt_bwd_delta(Geo geo, T4 o, T4 d_o, T4 og, T4 d_og,
 }
 
 // ----------------------------------------------------------------------------------------------
-// backward pass 1 (query-stationary): dq, d_bias_table.  Same tiling as simt_fwd_local.
+// backward pass 1 (query-stationary): dq, and with the bias table (TAB) its gradient.  Same tiling as simt_fwd_local.
+// TAB: as wg_bwd_dq, the CTA is slice cid.b of the images and runs images cid.b, cid.b + nslice, ...; the dS of each
+// chunk piece go to a tile and are added in a fixed order to the CTA's row of table partials tpart (table_grad_piece).
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, bool DROP = false>
-__global__ void __launch_bounds__(128)
+constexpr int kSimtDsLd = 65;   // dS tile row stride: the 16 query slots of a warp write one column in distinct banks
+inline size_t simt_ds_tile_bytes() { return 64 * kSimtDsLd * sizeof(float); }
+
+template <typename T, int HD, bool DROP = false, bool TAB = false>
+__global__ void __launch_bounds__(128, TAB && HD <= 8 ? 4 : 0)
 simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse,
             const float* __restrict__ delta, const float* __restrict__ table,
-            const float* __restrict__ g2l, float* __restrict__ d_table) {
+            const float* __restrict__ g2l, float* __restrict__ tpart) {
   using TL = Tile<HD>;
   constexpr int HH = TL::HH, HS = TL::HS;
   extern __shared__ float smem[];
@@ -339,12 +344,20 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
   short* kvr = reinterpret_cast<short*>(tab + tabn);
   short* kvc = kvr + 64;
   unsigned char* kfl = reinterpret_cast<unsigned char*>(kvc + 64);
+  float* dst = nullptr;                                   // TAB: the dS tile, 16-byte aligned after kfl
+  float* acc = nullptr;                                   // TAB: the CTA's row of table partials
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
+  const int h = cid.h, R = cid.R, C = cid.C;
   const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
   const int w = geo.w, D = geo.D;
   for (int i = tid; i < tabn; i += 128) tab[i] = table[(long long)i * geo.H + h];
+  if constexpr (TAB) {
+    dst = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(smem) +
+                                   ((reinterpret_cast<unsigned char*>(kfl + 64) - reinterpret_cast<unsigned char*>(smem) + 15) & ~15));
+    acc = tpart + (long long)blockIdx.x * tabn;
+    for (int i = tid; i < tabn; i += 128) acc[i] = 0.f;
+  }
 
   const int l = cid.piece * 64 + slot;
   const int qr = l / w, qc = l % w;
@@ -352,6 +365,9 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
   const bool qvalid = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
   const long long tokq = (long long)r * geo.ny + c;
 
+  const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
+  for (int it = 0; it < nimg; ++it) {
+  const int b = cid.b + it * geo.nslice;
   float qh[HH], doh[HH], dqh[HH];
 #pragma unroll
   for (int i = 0; i < HH; ++i) { qh[i] = 0.f; doh[i] = 0.f; dqh[i] = 0.f; }
@@ -416,7 +432,10 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
     __syncthreads();
     for (int j = 0; j < 64; ++j) {
       const int f = kfl[j];
-      if (!f) continue;
+      if (!f) {
+        if (TAB && half == 0) dst[slot * kSimtDsLd + j] = 0.f;
+        continue;
+      }
       float km = 1.f;                                    // dropout: keep / (1 - p) of the column
       if constexpr (DROP) km = drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? geo.drop_scale : 0.f;
       const float* kd = Ks + j * HS + TL::off(half);
@@ -434,14 +453,21 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
         if (geo.exact == 1 && (abs(dr) > w || abs(dc) > w)) ok = false;
         if (geo.has_bias && ok) { bidx = (dr + 2 * w - 1) * tw + dc + 2 * w - 1; bias = tab[bidx]; }
       }
+      float tg = 0.f;                                    // TAB: this pair's term of the table gradient
       if (ok) {
         const float p = __expf(fmaf(geo.scale, sp, bias) - lse_i);
         if constexpr (DROP) dpp *= km;
         const float ds = p * (dpp - del_i);
 #pragma unroll
         for (int i = 0; i < HH; ++i) dqh[i] = fmaf(ds, kd[i], dqh[i]);
-        if (bidx >= 0 && half == 0 && d_table != nullptr)
-          atomicAdd(d_table + (long long)bidx * geo.H + h, ds);
+        if (bidx >= 0) tg = ds;
+      }
+      if (TAB && half == 0) dst[slot * kSimtDsLd + j] = tg;
+    }
+    if constexpr (TAB) {
+      if (!isg) {            // CTA-uniform; the next piece writes the tile only after its two barriers
+        __syncthreads();     // every query's dS is in the tile
+        table_grad_piece(dst, kSimtDsLd, acc, geo, dR, dC, cid.piece, kp);
       }
     }
   }
@@ -449,6 +475,7 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
 #pragma unroll
     for (int i = 0; i < HH; ++i) dqh[i] *= geo.scale;
     store_seg<T, HH>(row_ptr_w<T>(dq, b, h, tokq), half * HH, D, dqh);
+  }
   }
 }
 
@@ -584,13 +611,14 @@ __device__ __forceinline__ float block_sum_256(float v, float* red /*[8]*/) {
 }
 
 // ----------------------------------------------------------------------------------------------
-// backward, global KEY columns seen by the local queries: dk[t], dv[t] for t < nglo and d_g2l[1][h][t].
+// backward, global KEY columns seen by the local queries: dk[t], dv[t] for t < nglo and, with the bias table, this
+// image's term of d_g2l[1][h][t] into pcol[b][h][t] (summed over the images by simt_bwd_bias_reduce).
 // CTA = one (b, h, t); row groups stride over the local queries.
 // ----------------------------------------------------------------------------------------------
 template <typename T, int HD, typename TO = T, bool DROP = false>
 __global__ void __launch_bounds__(256)
 simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
-              const float* __restrict__ delta, const float* __restrict__ g2l, float* __restrict__ d_g2l) {
+              const float* __restrict__ delta, const float* __restrict__ g2l, float* __restrict__ pcol) {
   constexpr int LPR = HD / 8, RPW = 32 / LPR, ROWS = 8 * RPW;
   __shared__ float red[8];
   __shared__ float accs[8][2][HD];
@@ -646,11 +674,12 @@ simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
     row_ptr_w<TO>(dk, b, h, t)[tid] = ElemTraits<TO>::from_f(x * geo.scale);
     row_ptr_w<TO>(dv, b, h, t)[tid] = ElemTraits<TO>::from_f(y);
   }
-  if (tid == 0 && geo.has_bias && d_g2l != nullptr) atomicAdd(d_g2l + ((long long)geo.H + h) * geo.g + t, tb);
+  if (tid == 0 && geo.has_bias) pcol[((long long)b * geo.H + h) * geo.g + t] = tb;
 }
 
 // ----------------------------------------------------------------------------------------------
-// backward, global QUERY rows: dqg, contributions to dkg / dvg over all N keys, d_g2g, d_g2l[0].
+// backward, global QUERY rows: dqg, contributions to dkg / dvg over all N keys, and with the bias table this image's
+// terms of d_g2g into pgg[b][h][a][j] and of d_g2l[0] into prow[b][h][a] (summed over the images by simt_bwd_bias_reduce).
 // CTA = one (b, h); row groups stride over the keys.  `accumulate` != 0: add into dkg/dvg (they alias dk/dv,
 // already written by the dK/dV pass and simt_bwd_gcol earlier on the same stream); else overwrite.
 // ----------------------------------------------------------------------------------------------
@@ -659,7 +688,7 @@ __global__ void __launch_bounds__(256)
 simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
               const float* __restrict__ lse_g, const float* __restrict__ delta_g,
               const float* __restrict__ g2l, const float* __restrict__ g2g,
-              float* __restrict__ d_g2l, float* __restrict__ d_g2g, int accumulate, int rmw_rows) {
+              float* __restrict__ prow, float* __restrict__ pgg, int accumulate, int rmw_rows) {
   // rmw_rows: keys [0, rmw_rows) get their dkg / dvg rows updated here
   constexpr int LPR = HD / 8, RPW = 32 / LPR, ROWS = 8 * RPW;
   __shared__ float red[8];
@@ -702,8 +731,8 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
       if constexpr (DROP) km = drop_keep(geo, (uint32_t)a, (uint32_t)jc, 2u * (uint32_t)(b * geo.H + h) + 1u) ? geo.drop_scale : 0.f;
       const float ds = DROP ? p * (dpp * km - dg) : p * (dpp - dg);
       const float pv = DROP ? p * km : p;
-      if (geo.has_bias && valid && sub == 0) {
-        if (j < geo.g) { if (d_g2g) atomicAdd(d_g2g + ((long long)h * geo.g + a) * geo.g + j, ds); }
+      if (geo.has_bias && valid && sub == 0) {   // each j < g is one row group's, once per a
+        if (j < geo.g) pgg[(((long long)b * geo.H + h) * geo.g + a) * geo.g + j] = ds;
         else adb += ds;
       }
       const float dss = ds * geo.scale;
@@ -731,7 +760,46 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
       for (int w2 = 0; w2 < 8; ++w2) x += accs[w2][tid];
       row_ptr_w<TO>(dqg, b, h, a)[tid] = ElemTraits<TO>::from_f(x * geo.scale);
     }
-    if (tid == 0 && geo.has_bias && d_g2l != nullptr) atomicAdd(d_g2l + (long long)h * geo.g + a, tb);
+    if (tid == 0 && geo.has_bias) prow[((long long)b * geo.H + h) * geo.g + a] = tb;
+  }
+}
+
+// ----------------------------------------------------------------------------------------------
+// backward, bias gradients: every partial summed in a fixed order and added into the caller's tensors.  Thread x < ntab:
+// d_bias_table entry e of head h (x = h tabn + e) over the pass-1 CTAs of h, slice by slice; then (x - ntab < nglob) the
+// global-bias entries over the images.  ntab / nglob are 0 when the kernel that writes those partials did not run.
+// ----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+simt_bwd_bias_reduce(Geo geo, const float* __restrict__ tpart, const float* __restrict__ gpart, float* __restrict__ d_table,
+                     float* __restrict__ d_g2l, float* __restrict__ d_g2g, int ntab, int nglob) {
+  long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int H = geo.H;
+  float sum = 0.f;
+  if (x < ntab) {
+    const int tabn = ntab / H, h = (int)(x / tabn), e = (int)(x % tabn);
+    const long long m = (long long)geo.mx * geo.my * geo.npc;   // pass-1 CTAs of one (slice, head)
+    for (int s = 0; s < geo.nslice; ++s) {
+      const float* p = tpart + ((long long)s * H + h) * m * tabn + e;
+#pragma unroll 4
+      for (long long c = 0; c < m; ++c) sum += p[c * tabn];
+    }
+    d_table[(long long)e * H + h] += sum;
+    return;
+  }
+  x -= ntab;
+  if (x >= nglob) return;
+  const long long hg = (long long)H * geo.g, bhg = (long long)geo.B * hg;
+  if (x < 2 * hg) {          // d_g2l[1] (simt_bwd_gcol), then d_g2l[0] (simt_bwd_grow); x % hg = h g + t
+    const int part = x < hg ? 0 : 1;
+    const long long i = x - part * hg;
+    const float* p = gpart + part * bhg + i;
+    for (int b = 0; b < geo.B; ++b) sum += p[b * hg];
+    if (d_g2l != nullptr) d_g2l[(part == 0 ? hg : 0) + i] += sum;
+  } else {                   // d_g2g: i = (h g + a) g + j
+    const long long i = x - 2 * hg;
+    const float* p = gpart + 2 * bhg + i;
+    for (int b = 0; b < geo.B; ++b) sum += p[b * hg * geo.g];
+    if (d_g2g != nullptr) d_g2g[i] += sum;
   }
 }
 
@@ -745,16 +813,21 @@ inline void launch_global_fwd_kernels(const Geo& g, T4 qg, T4 kg, T4 vg, T4 og, 
 template <typename T, int HD, typename TO = T>
 inline void launch_global_bwd_kernels(const Geo& g, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, T4 qg, T4 kg, T4 vg, T4 d_og,
                                       T4 dqg, T4 dkg, T4 dvg, const float* lse, const float* delta, const float* lse_g,
-                                      const float* delta_g, const float* g2l, const float* g2g, float* d_g2l,
-                                      float* d_g2g, int accumulate, int rmw_rows, cudaStream_t s) {
+                                      const float* delta_g, const float* g2l, const float* g2g, float* gpart,
+                                      int accumulate, int rmw_rows, cudaStream_t s) {
+  // gpart: the global-bias partials (vil_common.cuh, ws_off_glob), read only with the bias table
+  const long long bhg = (long long)g.B * g.H * g.g;
+  float* pcol = gpart;
+  float* prow = gpart ? gpart + bhg : nullptr;
+  float* pgg = gpart ? gpart + 2 * bhg : nullptr;
   if (g.drop_p > 0.f) {
-    simt_bwd_gcol<T, HD, TO, true><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, d_g2l);
-    simt_bwd_grow<T, HD, TO, true><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, d_g2l,
-                                                             d_g2g, accumulate, rmw_rows);
+    simt_bwd_gcol<T, HD, TO, true><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, pcol);
+    simt_bwd_grow<T, HD, TO, true><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, prow,
+                                                             pgg, accumulate, rmw_rows);
     return;
   }
-  simt_bwd_gcol<T, HD, TO><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, d_g2l);
-  simt_bwd_grow<T, HD, TO><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, d_g2l, d_g2g,
+  simt_bwd_gcol<T, HD, TO><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, pcol);
+  simt_bwd_grow<T, HD, TO><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, prow, pgg,
                                                   accumulate, rmw_rows);
 }
 

@@ -30,6 +30,8 @@ const char* why_not(const VilAttnParams* p, const Geo& g, bool bwd) {
   if (g.D % 8 != 0 || !rows_aligned16(p->q) || !rows_aligned16(p->k) || !rows_aligned16(p->v) || (bwd && !rows_aligned16(p->d_o)))
     return "q / k / v / d_o rows are not 16-byte aligned (D % 8 != 0, or a pointer or b / h / t stride off 16 bytes)";
   if (wg::DkvSmem<64>::total(table_floats(g)) > 227 * 1024) return "bias table does not fit in shared memory";
+  if (bwd && g.has_bias && wg::DqSmem<64>::total(table_floats(g), true) > 227 * 1024)
+    return "bias table and the dS tile of its gradient do not fit in shared memory";
   return nullptr;
 }
 
@@ -50,6 +52,20 @@ int forward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   return VIL_OK;
 }
 
+// backward pass 1; TAB (the bias table): nslice image slices per (head, chunk, piece), table partials into the workspace
+template <typename T, int HD, typename TO, bool DROP, bool TAB>
+int dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+  int rc;
+  const size_t sm = wg::DqSmem<HD>::total(table_floats(g), TAB);
+  if ((rc = set_smem(wg::wg_bwd_dq<T, HD, TO, DROP, TAB>, sm))) return rc;
+  const long long ctas = TAB ? tab_ctas(g) : blocks(g);
+  wg::wg_bwd_dq<T, HD, TO, DROP, TAB><<<(unsigned)ctas, wg::kThreads, sm, s>>>(
+      g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse, ws_at(p, 0), p->bias_table, p->g2l,
+      TAB ? ws_at(p, ws_off_tab(g)) : nullptr);
+  count_launch();
+  return launch_check("wgmma_bwd_dq");
+}
+
 template <typename T, int HD, typename TO, bool DROP>
 int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   int rc;
@@ -57,12 +73,7 @@ int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   float* delta = static_cast<float*>(p->workspace);
   const int tabn = table_floats(g);
   if (!(p->skip_mask & 2)) {
-    const size_t sm = wg::DqSmem<HD>::total(tabn);
-    if ((rc = set_smem(wg::wg_bwd_dq<T, HD, TO, DROP>, sm))) return rc;
-    wg::wg_bwd_dq<T, HD, TO, DROP><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq),
-                                                                         p->lse, delta, p->bias_table, p->g2l, p->d_bias_table);
-    count_launch();
-    if ((rc = launch_check("wgmma_bwd_dq"))) return rc;
+    if ((rc = g.has_bias ? dq_pass<T, HD, TO, DROP, true>(p, g, s) : dq_pass<T, HD, TO, DROP, false>(p, g, s))) return rc;
   }
   if (!(p->skip_mask & 4)) {
     const size_t sm = wg::DkvSmem<HD>::total(tabn, DROP);
@@ -72,8 +83,8 @@ int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
     count_launch();
     if ((rc = launch_check("wgmma_bwd_dkv"))) return rc;
   }
-  if (g.g > 0 && !(p->skip_mask & 1)) return simt_global_bwd(p, g, s, g.N);
-  return VIL_OK;
+  if (g.g > 0 && !(p->skip_mask & 1) && (rc = simt_global_bwd(p, g, s, g.N))) return rc;
+  return simt_bias_reduce(p, g, s);
 }
 
 template <typename T, typename TO, bool DROP>

@@ -259,22 +259,30 @@ __device__ __forceinline__ void fwd_scores(float (&s)[32], float (&mx)[2], const
   }
 }
 
-// pass 1: dS = P (dP - delta) of one piece into s, and the bias-table gradient when d_table is set.  Rows past the chunk
-// carry lse = +inf, so their P is 0.
+// pass 1: dS = P (dP - delta) of one piece into s.  Rows past the chunk carry lse = +inf, so their P is 0.  With the bias
+// table (RPE) the dS that enter its gradient also go to the fp32 tile dst (row stride kDsLd); every other element of the
+// tile gets 0.
+constexpr int kDsLd = 72;   // a row of 64 + 8: the float2 stores of a warp's 8 rows x 4 column pairs fall in distinct banks
+constexpr size_t kDsTile = 64 * kDsLd * sizeof(float);
+
 template <bool RPE, bool WIN>
 __device__ __forceinline__ void dq_scores(float (&s)[32], const float (&dp)[32], const Geo& geo, const KeyCols& kc,
                                           const float* tab, const QRows& q, int gl, const float (&lse_r)[2],
-                                          const float (&del_r)[2], float* __restrict__ d_table, int h) {
+                                          const float (&del_r)[2], float* __restrict__ dst) {
   int tb[2] = {0, 0};
   if (RPE) row_tix(geo, q, tb);
+  float prev = 0.f;
 #pragma unroll
   for (int i = 0; i < 32; ++i) {
     const int e = (i >> 1) & 1;
     int bidx;
     const float val = key_score<RPE, WIN>(geo, kc, tab, q, tb, e, acc_col(i), gl, s[i], bidx);
     const float ds = __expf(val - lse_r[e]) * (dp[i] - del_r[e]);
-    if (RPE && d_table != nullptr && bidx >= 0 && q.ok[e] && val != -INFINITY)
-      atomicAdd(d_table + (long long)bidx * geo.H + h, ds);
+    if (RPE) {
+      const float t = (bidx >= 0 && q.ok[e] && val != -INFINITY) ? ds : 0.f;
+      if (i & 1) *reinterpret_cast<float2*>(dst + acc_row(i) * kDsLd + acc_col(i - 1)) = make_float2(prev, t);
+      prev = t;
+    }
     s[i] = ds;
   }
 }
@@ -300,9 +308,11 @@ template <int HD> struct FwdSmem {     // Q; K, V per stage
   static constexpr size_t tiles = (1 + 2 * kStages) * 64 * HD * 2;
   static size_t total(int tabn) { return (tiles + kStages * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
 };
-template <int HD> struct DqSmem {      // Q, dO; K, V per stage
+template <int HD> struct DqSmem {      // Q, dO; K, V per stage; with the bias table, the dS tile after the table
   static constexpr size_t tiles = (2 + 2 * kStages) * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + kStages * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
+  static size_t total(int tabn, bool tab = false) {
+    return ((tiles + kStages * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15)) + (tab ? kDsTile : 0);
+  }
 };
 template <int HD> struct DkvSmem {     // K, V; Q, dO per stage; the key rows' chunk positions
   static constexpr size_t tiles = (2 + 2 * kStages) * 64 * HD * 2;
@@ -456,10 +466,13 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
 // ----------------------------------------------------------------------------------------------
 // backward pass 1 (query-stationary): dq and the local-bias-table gradient
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO, bool DROP = false>
+// TAB (the call has the bias table): the CTA is slice cid.b of the images and runs images cid.b, cid.b + nslice, ...;
+// after each chunk piece's dQ product its dS tile is added, in a fixed order, to the CTA's row of table partials tpart
+// (vil_common.cuh: table_grad_piece).  Without TAB, one image per CTA and none of that code.
+template <typename T, int HD, typename TO, bool DROP = false, bool TAB = false>
 __global__ void __launch_bounds__(kThreads)
 wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse, const float* __restrict__ delta,
-          const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ d_table) {
+          const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ tpart) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
   using W64 = sm90::Wg<T, 64>;
   using WHD = sm90::Wg<T, HD>;
@@ -470,14 +483,25 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages * TILE);
   Visit* vl = reinterpret_cast<Visit*>(meta + kStages * kKeyCols);
   float* tab = reinterpret_cast<float*>(vl + 9);
-  const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
+  const int tabn = TAB ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
+  float* dst = nullptr;                                           // TAB: the dS tile, 16-byte aligned after the table
+  float* acc = nullptr;                                           // TAB: the CTA's row of table partials
 
   const Cta cid = decode(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
+  const int h = cid.h, R = cid.R, C = cid.C;
   const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
   const int w = geo.w, D = geo.D;
-  const long long bh = (long long)b * geo.H + h;
   for (int i = tid; i < tabn; i += kThreads) tab[i] = table[(long long)i * geo.H + h];
+  if constexpr (TAB) {
+    dst = reinterpret_cast<float*>(smem_raw + ((reinterpret_cast<unsigned char*>(tab + tabn) - smem_raw + 15) & ~15));
+    acc = tpart + (long long)blockIdx.x * tabn;
+    for (int i = tid; i < tabn; i += kThreads) acc[i] = 0.f;
+  }
+  const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
+  for (int it = 0; it < nimg; ++it) {
+  const int b = cid.b + it * geo.nslice;
+  const long long bh = (long long)b * geo.H + h;
+  if (TAB && it > 0) __syncthreads();                             // the previous image is done with Qs, Gs, vl and the tile
   {
     const int l = cid.piece * 64 + slot;
     const int r = R * w + l / w, c = C * w + l % w;
@@ -501,7 +525,6 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   for (int i = 0; i < HH; ++i) dqacc[i] = 0.f;
 
   const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, R, C, 1, vl) * geo.npc;
-  const int epi = key_epilogue(geo);
   const T* kb = row_ptr<T>(k, b, h, 0);
   const T* vb = row_ptr<T>(v, b, h, 0);
   SlotWalk wk(geo, slot);
@@ -532,12 +555,9 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
       drop_rows(geo, R, C, cid.piece, drow);
       drop_key_piece(dp, geo, drow, drop_col_base(geo, vl, ngp, pi), 2u * (uint32_t)(b * geo.H + h), geo.drop_scale);
     }
-    switch (epi) {   // CTA-uniform
-      case 0: dq_scores<false, false>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
-      case 1: dq_scores<false, true>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
-      case 2: dq_scores<true, false>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
-      default: dq_scores<true, true>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, d_table, h); break;
-    }
+    // CTA-uniform: the bias-table forms run only in the TAB instantiation
+    if (geo.exact == 1) dq_scores<TAB, true>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, dst);
+    else dq_scores<TAB, false>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, dst);
     uint32_t a[4][4];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) to_a_frag<T>(s, kk, a[kk]);
@@ -547,12 +567,20 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(dqacc);
+    if constexpr (TAB) {
+      if (pi >= ngp) {       // a chunk piece (CTA-uniform); the tile is rewritten only after the next round's barrier
+        __syncthreads();     // every thread's dS is in the tile
+        const int c = pi - ngp, vi = c / geo.npc;
+        table_grad_piece(dst, kDsLd, acc, geo, vl[vi].dR, vl[vi].dC, cid.piece, c - vi * geo.npc);
+      }
+    }
   }
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     if (!qrow.ok[e]) continue;
     const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
     store_rows<TO, HD>(dqacc, e, row_ptr_w<TO>(dq, b, h, tokq), D, geo.scale);
+  }
   }
 }
 

@@ -9,6 +9,9 @@ the reference tree does not exist; module / parameter names follow the reference
 so its checkpoints load unchanged (pinned by tests/test_msvit_harness.py against
 golden vectors generated from the reference).
 
+With dense_impl="vil" and the longformer stages on the fused operator, the attention backward is deterministic, rpe
+on or off (include/vil_attn.h), so a training step repeats bit for bit under torch.use_deterministic_algorithms(True).
+
 Arch string grammar (msvit.py:402-410): stages separated by `_`, fields by `,`:
   l<stage id> h<heads> d<dim> n<blocks> s<1: longformer attention, 0: dense>
   g<global tokens> p<patch size> f<window w> a<1: absolute pos-embed, 0: relative bias>

@@ -7,6 +7,11 @@ consumes the outputs of the `query` / `kv` Linears *in place* (no transposes or
 .contiguous() copies, cf. longformer2d.py:126-149) and writes the attention
 output directly in (B, N, H*D) layout for `proj` (cf. :201-203).
 
+The backward is deterministic: identical inputs give bitwise-identical gradients on a given build and GPU model,
+including those of the relative-position-bias parameters (summed in a fixed order, no atomics), so it needs no special
+handling under torch.use_deterministic_algorithms(True).  The workspace is sized by vil_attn_workspace_bytes, which
+includes the bias-gradient partials when the table is given.
+
 Replaces: longformer2d.py:126-202 + :210-226 and everything in
 slidingchunk_2d.py they call.
 """
