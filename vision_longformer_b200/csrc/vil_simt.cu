@@ -68,13 +68,6 @@ int global_bwd_t(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_r
     case 64:  return CALL(T, 64, TO);                              \
     default:  return CALL(T, 128, TO);                             \
   }
-#define VIL_SIMT_HD64(T, TO, CALL)                                 \
-  switch (head_bucket(g.D)) {                                      \
-    case 8:   return CALL(T, 8, TO);                               \
-    case 16:  return CALL(T, 16, TO);                              \
-    case 32:  return CALL(T, 32, TO);                              \
-    default:  return CALL(T, 64, TO);                              \
-  }
 #define VIL_SIMT_TYPES(HDM, CALL)                                                                   \
   if (p->dtype == VIL_F32) { HDM(float, float, CALL) }                                         \
   if (p->dtype == VIL_BF16) {                                                                  \
@@ -122,8 +115,10 @@ int simt_dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
 
 template <typename T, int HD, bool DROP>
 int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
-  if constexpr (HD > 64) {
-    return shared_fail(VIL_E_UNSUPPORTED, "backward supports head dim <= 64");
+  if constexpr (HD > 64) {   // two threads per row would hold 4 x 64 fp32 values in pass 2
+    return shared_fail(VIL_E_UNSUPPORTED,
+                       "the SIMT backward supports head dim <= 64; 64 < D <= 128 is trained by the wgmma family "
+                       "(bf16 / fp16 with 16-byte-aligned rows)");
   } else {
     int rc = (p->skip_mask & 8) ? VIL_OK : delta_t<T, T>(p, g, s);
     if (rc) return rc;
@@ -199,9 +194,8 @@ int simt_bias_reduce(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
 }
 
 int simt_global_bwd(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_rows) {
-  if (g.D > 64) return shared_fail(VIL_E_UNSUPPORTED, "backward supports head dim <= 64");
 #define CALL_GB(T, HD, TO) global_bwd_t<T, HD, TO>(p, g, s, rmw_rows)
-  VIL_SIMT_TYPES(VIL_SIMT_HD64, CALL_GB)
+  VIL_SIMT_TYPES(VIL_SIMT_HD, CALL_GB)
 #undef CALL_GB
 }
 

@@ -1,10 +1,11 @@
 // SIMT (CUDA-core, fp32 accumulate) kernel family of the Vision-Longformer attention.
 //
 // Covers EVERY configuration of the reference operator (any w, exact in {0,1,-1},
-// mode in {-1,0,1..8}, any nglo, D <= 128 forward / D <= 64 backward, fp32 / bf16 /
-// fp16 I/O).  It is (a) the fp32 parity build (1e-5 vs the fp64 oracle), (b) the
-// path for configurations the wgmma family does not cover, and (c) the home of
-// the small global-token kernels that both families share.
+// mode in {-1,0,1..8}, any nglo, D <= 128 forward / D <= 64 backward and dropout,
+// fp32 / bf16 / fp16 I/O).  It is (a) the fp32 parity build (1e-5 vs the fp64 oracle),
+// (b) the path for configurations the wgmma family does not cover, and (c) the home of
+// the small global-token kernels that both families share (every D <= 128: bf16 / fp16
+// training at 64 < D <= 128 runs on the wgmma family and these kernels).
 //
 // Math restated from the reference (closed forms verified in oracle/vil_oracle.py):
 //   local query i=(r_i,c_i) in chunk (R,C); for every visited chunk offset (dR,dC)

@@ -7,7 +7,7 @@
 namespace vil {
 namespace {
 
-int head_tile(int D) { return D <= 16 ? 16 : D <= 32 ? 32 : 64; }
+int head_tile(int D) { return D <= 16 ? 16 : D <= 32 ? 32 : D <= 64 ? 64 : 128; }
 int table_floats(const Geo& g) { return g.has_bias ? (4 * g.w - 1) * (4 * g.w - 1) : 0; }
 
 template <typename K>
@@ -24,15 +24,30 @@ bool rows_aligned16(const VilTensor4& t) {
   return reinterpret_cast<uintptr_t>(t.ptr) % 16 == 0 && (t.sb * e) % 16 == 0 && (t.sh * e) % 16 == 0 && (t.st * e) % 16 == 0;
 }
 
-const char* why_not(const VilAttnParams* p, const Geo& g, bool bwd) {
-  if (p->dtype != VIL_BF16 && p->dtype != VIL_F16) return "dtype is fp32 (wgmma operands are bf16 / fp16)";
-  if (g.D > 64) return "head dim > 64";
-  if (g.D % 8 != 0 || !rows_aligned16(p->q) || !rows_aligned16(p->k) || !rows_aligned16(p->v) || (bwd && !rows_aligned16(p->d_o)))
-    return "q / k / v / d_o rows are not 16-byte aligned (D % 8 != 0, or a pointer or b / h / t stride off 16 bytes)";
-  if (wg::DkvSmem<64>::total(table_floats(g)) > 227 * 1024) return "bias table does not fit in shared memory";
-  if (bwd && g.has_bias && wg::DqSmem<64>::total(table_floats(g), true) > 227 * 1024)
+// Shared memory of the call's kernels at head tile HD beside its bias table.  Every call checks all three kernels, so that
+// a forward runs on this family only if its backward can as well.  Up to HD 64 everything fits up to the largest window
+// (w = 48); at HD 128 the bias table fits up to w = 42, limited by pass 1 with its dS tile (DESIGN.md section 3).
+template <int HD>
+const char* smem_why_not(const Geo& g) {
+  constexpr size_t cap = 227 * 1024;
+  const int tabn = table_floats(g);
+  if (wg::FwdSmem<HD>::total(tabn) > cap || wg::DkvSmem<HD>::total(tabn, g.drop_p > 0.f) > cap)
+    return "bias table does not fit in shared memory";
+  if (g.has_bias && wg::DqSmem<HD>::total(tabn, true) > cap)
     return "bias table and the dS tile of its gradient do not fit in shared memory";
   return nullptr;
+}
+
+const char* why_not(const VilAttnParams* p, const Geo& g, bool bwd) {
+  if (p->dtype != VIL_BF16 && p->dtype != VIL_F16) return "dtype is fp32 (wgmma operands are bf16 / fp16)";
+  if (g.D % 8 != 0 || !rows_aligned16(p->q) || !rows_aligned16(p->k) || !rows_aligned16(p->v) || (bwd && !rows_aligned16(p->d_o)))
+    return "q / k / v / d_o rows are not 16-byte aligned (D % 8 != 0, or a pointer or b / h / t stride off 16 bytes)";
+  switch (head_tile(g.D)) {
+    case 16: return smem_why_not<16>(g);
+    case 32: return smem_why_not<32>(g);
+    case 64: return smem_why_not<64>(g);
+    default: return smem_why_not<128>(g);
+  }
 }
 
 long long blocks(const Geo& g) { return (long long)g.B * g.H * g.mx * g.my * g.npc; }
@@ -92,7 +107,8 @@ int dispatch_hd_drop(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool 
   switch (head_tile(g.D)) {
     case 16: return bwd ? backward_t<T, 16, TO, DROP>(p, g, s) : forward_t<T, 16, TO, DROP>(p, g, s);
     case 32: return bwd ? backward_t<T, 32, TO, DROP>(p, g, s) : forward_t<T, 32, TO, DROP>(p, g, s);
-    default: return bwd ? backward_t<T, 64, TO, DROP>(p, g, s) : forward_t<T, 64, TO, DROP>(p, g, s);
+    case 64: return bwd ? backward_t<T, 64, TO, DROP>(p, g, s) : forward_t<T, 64, TO, DROP>(p, g, s);
+    default: return bwd ? backward_t<T, 128, TO, DROP>(p, g, s) : forward_t<T, 128, TO, DROP>(p, g, s);
   }
 }
 

@@ -15,6 +15,7 @@
 // product (V, K, dO, Q: consumed along the token axis) is the same (token, d) tile an SS product reads K-major, read
 // MN-major.
 #pragma once
+#include <type_traits>
 #include "vil_common.cuh"
 #include "vil_sm90.cuh"
 
@@ -38,9 +39,10 @@ __device__ __forceinline__ Cta decode(const Geo& g, int bid) {
 __device__ __forceinline__ int acc_row(int i) { return ((threadIdx.x >> 5) << 4) + ((threadIdx.x & 31) >> 2) + (((i >> 1) & 1) << 3); }
 __device__ __forceinline__ int acc_col(int i) { return ((i >> 2) << 3) + ((threadIdx.x & 3) << 1) + (i & 1); }
 
-// Ring of operand stages: piece pi is staged into stage pi % kStages while the pieces before it are multiplied, so the
-// copies of kStages - 1 pieces are in flight behind the MMAs of a round.
-constexpr int kStages = 3;
+// Ring of operand stages: piece pi is staged into stage pi % kStages<HD> while the pieces before it are multiplied, so the
+// copies of kStages<HD> - 1 pieces are in flight behind the MMAs of a round.  3 stages up to HD 64; at HD 128 a stage is
+// two 16 KB tiles and 2 stages keep two CTAs on an SM (3 would leave one, DESIGN.md section 3).
+template <int HD> constexpr int kStages = HD <= 64 ? 3 : 2;
 
 // The thread's row segment of a (64 x HD) tile: row `row`, columns [half HD / 2, (half + 1) HD / 2), copied 16 bytes at a
 // time from row `tok` of the (b, h) slice `base` (row stride st) straight into the core-matrix layout.  tok < 0 (a phantom
@@ -150,6 +152,19 @@ struct SlotWalk {
   __device__ __forceinline__ void next(const Geo& geo) {
     if (++pj == geo.npc) { pj = 0; ++vi; kr = r0; kc = c0; return; }
     kr += dr; kc += dc;
+    if (kc >= geo.w) { kc -= geo.w; ++kr; }
+  }
+};
+
+// SlotWalk holding only the position: the start and the step are recomputed (two divisions per piece) rather than kept
+// in registers across the loop.  Pass 2 at HD 128 uses it: its 128 accumulator registers leave none to spare.
+struct SlotWalkLean {
+  int vi, pj, kr, kc;
+  __device__ __forceinline__ SlotWalkLean(const Geo& geo, int slot) : vi(0), pj(0), kr(slot / geo.w), kc(slot % geo.w) {}
+  __device__ __forceinline__ void next(const Geo& geo) {
+    const int slot = threadIdx.x >> 1;
+    if (++pj == geo.npc) { pj = 0; ++vi; kr = slot / geo.w; kc = slot % geo.w; return; }
+    kr += 64 / geo.w; kc += 64 % geo.w;
     if (kc >= geo.w) { kc -= geo.w; ++kr; }
   }
 };
@@ -287,7 +302,7 @@ __device__ __forceinline__ void dq_scores(float (&s)[32], const float (&dp)[32],
   }
 }
 
-// Shared memory of a CTA: the stationary tiles, kStages stages of two streamed tiles each, kStages sets of per-column
+// Shared memory of a CTA: the stationary tiles, kStages<HD> stages of two streamed tiles each, as many sets of per-column
 // metadata, the visit list and the bias table.
 constexpr size_t kKeyCols = 64 * (4 + 4 + 2 + 2);
 constexpr size_t kQueryCols = 64 * (4 + 4 + 4 + 2 + 2 + 1);
@@ -305,30 +320,30 @@ __device__ __forceinline__ KeyCols key_cols(unsigned char* meta, int stage) {
 }
 
 template <int HD> struct FwdSmem {     // Q; K, V per stage
-  static constexpr size_t tiles = (1 + 2 * kStages) * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + kStages * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
+  static constexpr size_t tiles = (1 + 2 * kStages<HD>) * 64 * HD * 2;
+  static size_t total(int tabn) { return (tiles + kStages<HD> * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
 };
 template <int HD> struct DqSmem {      // Q, dO; K, V per stage; with the bias table, the dS tile after the table
-  static constexpr size_t tiles = (2 + 2 * kStages) * 64 * HD * 2;
+  static constexpr size_t tiles = (2 + 2 * kStages<HD>) * 64 * HD * 2;
   static size_t total(int tabn, bool tab = false) {
-    return ((tiles + kStages * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15)) + (tab ? kDsTile : 0);
+    return ((tiles + kStages<HD> * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15)) + (tab ? kDsTile : 0);
   }
 };
 template <int HD> struct DkvSmem {     // K, V; Q, dO per stage; the key rows' chunk positions
-  static constexpr size_t tiles = (2 + 2 * kStages) * 64 * HD * 2;
+  static constexpr size_t tiles = (2 + 2 * kStages<HD>) * 64 * HD * 2;
   static size_t total(int tabn, bool drop = false) {
-    return (tiles + kStages * query_cols_bytes(drop) + kVisits + 64 * sizeof(int) + (size_t)tabn * 4 + 15) & ~size_t(15);
+    return (tiles + kStages<HD> * query_cols_bytes(drop) + kVisits + 64 * sizeof(int) + (size_t)tabn * 4 + 15) & ~size_t(15);
   }
 };
 
-// Stages key piece pi (K and V rows, the column metadata) into ring stage pi % kStages and commits it as one cp.async
+// Stages key piece pi (K and V rows, the column metadata) into ring stage pi % kStages<HD> and commits it as one cp.async
 // group; past the last piece it commits an empty group, so that every round waits on the same group count.
 template <typename T, int HD>
 __device__ __forceinline__ void issue_key_piece(const Geo& geo, int pi, int npieces, int ngp, const Visit* vl, SlotWalk& wk,
                                                 T* ring, unsigned char* meta, const T* kb, long long kst, const T* vb,
                                                 long long vst, int h, const float* __restrict__ g2l) {
   if (pi < npieces) {
-    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = pi % kStages;
+    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = pi % kStages<HD>;
     int gk, vr, vc;
     long long tok;
     bool ok;
@@ -343,8 +358,9 @@ __device__ __forceinline__ void issue_key_piece(const Geo& geo, int pi, int npie
 
 // Top of round pi: piece pi has landed in every thread's copies, is visible to the async proxy, and every thread is done
 // with round pi - 1, whose stage the next issue refills.
+template <int HD>
 __device__ __forceinline__ void ring_wait() {
-  sm90::cp_async_wait<kStages - 2>();
+  sm90::cp_async_wait<kStages<HD> - 2>();
   sm90::fence_proxy_async();
   __syncthreads();
 }
@@ -352,9 +368,10 @@ __device__ __forceinline__ void ring_wait() {
 // ----------------------------------------------------------------------------------------------
 // forward, local queries
 // ----------------------------------------------------------------------------------------------
-// held to 5 / 3 CTAs per SM (HD <= 32 / 64): left alone, ptxas spends registers on hoisting the column loads and drops one
+// held to 5 / 3 CTAs per SM (HD <= 32 / 64): left alone, ptxas spends registers on hoisting the column loads and drops one.
+// HD 128: 2, what the 2-stage ring fits (the O accumulator alone is 64 registers)
 template <typename T, int HD, typename TO, bool DROP = false>
-__global__ void __launch_bounds__(kThreads, HD <= 32 ? 5 : 3)
+__global__ void __launch_bounds__(kThreads, HD <= 32 ? 5 : HD <= 64 ? 3 : 2)
 wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const float* __restrict__ table,
              const float* __restrict__ g2l) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
@@ -363,8 +380,8 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* Qs = reinterpret_cast<T*>(smem_raw);
   T* ring = Qs + TILE;                                            // stage s: K at ring + 2 s TILE, V after it
-  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages * TILE);
-  Visit* vl = reinterpret_cast<Visit*>(meta + kStages * kKeyCols);
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages<HD> * TILE);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kStages<HD> * kKeyCols);
   float* tab = reinterpret_cast<float*>(vl + 9);
   const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
 
@@ -391,12 +408,12 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   SlotWalk wk(geo, slot);
   __syncthreads();                                                // the visit list
 #pragma unroll
-  for (int p = 0; p < kStages - 1; ++p)                           // the first group also carries Q
+  for (int p = 0; p < kStages<HD> - 1; ++p)                       // the first group also carries Q
     issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
   for (int pi = 0; pi < npieces; ++pi) {
-    ring_wait();
-    issue_key_piece<T, HD>(geo, pi + kStages - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
-    const int st = pi % kStages;
+    ring_wait<HD>();
+    issue_key_piece<T, HD>(geo, pi + kStages<HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    const int st = pi % kStages<HD>;
     const T* Ks = ring + st * 2 * TILE;
     const T* Vs = Ks + TILE;
     const KeyCols kcol = key_cols(meta, st);
@@ -469,8 +486,9 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
 // TAB (the call has the bias table): the CTA is slice cid.b of the images and runs images cid.b, cid.b + nslice, ...;
 // after each chunk piece's dQ product its dS tile is added, in a fixed order, to the CTA's row of table partials tpart
 // (vil_common.cuh: table_grad_piece).  Without TAB, one image per CTA and none of that code.
+// HD 128 is held to 2 CTAs per SM, what the 2-stage ring fits; below it ptxas is left alone.
 template <typename T, int HD, typename TO, bool DROP = false, bool TAB = false>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, HD <= 64 ? 0 : 2)
 wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse, const float* __restrict__ delta,
           const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ tpart) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
@@ -480,8 +498,8 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   T* Qs = reinterpret_cast<T*>(smem_raw);
   T* Gs = Qs + TILE;
   T* ring = Gs + TILE;                                            // stage s: K at ring + 2 s TILE, V after it
-  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages * TILE);
-  Visit* vl = reinterpret_cast<Visit*>(meta + kStages * kKeyCols);
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages<HD> * TILE);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kStages<HD> * kKeyCols);
   float* tab = reinterpret_cast<float*>(vl + 9);
   const int tabn = TAB ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
   float* dst = nullptr;                                           // TAB: the dS tile, 16-byte aligned after the table
@@ -530,12 +548,12 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   SlotWalk wk(geo, slot);
   __syncthreads();                                                // the visit list
 #pragma unroll
-  for (int p = 0; p < kStages - 1; ++p)                           // the first group also carries Q and dO
+  for (int p = 0; p < kStages<HD> - 1; ++p)                       // the first group also carries Q and dO
     issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
   for (int pi = 0; pi < npieces; ++pi) {
-    ring_wait();
-    issue_key_piece<T, HD>(geo, pi + kStages - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
-    const int st = pi % kStages;
+    ring_wait<HD>();
+    issue_key_piece<T, HD>(geo, pi + kStages<HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    const int st = pi % kStages<HD>;
     const T* Ks = ring + st * 2 * TILE;
     const T* Vs = Ks + TILE;
     const KeyCols kcol = key_cols(meta, st);
@@ -643,14 +661,14 @@ __device__ __forceinline__ QueryCols query_cols(unsigned char* meta, int stage, 
   return qc;
 }
 
-// Stages query piece qp (Q and dO rows, the column metadata with lse and delta) into ring stage qp % kStages and commits it
+// Stages query piece qp (Q and dO rows, the column metadata with lse and delta) into ring stage qp % kStages<HD> and commits it
 // as one cp.async group (an empty one past the last piece).  The walk runs over the chunks of vl, npc pieces each.
-template <typename T, int HD, bool DROP>
-__device__ __forceinline__ void issue_query_piece(const Geo& geo, int qp, int npieces, const Visit* vl, SlotWalk& wk, T* ring,
+template <typename T, int HD, bool DROP, typename Walk>
+__device__ __forceinline__ void issue_query_piece(const Geo& geo, int qp, int npieces, const Visit* vl, Walk& wk, T* ring,
                                                   unsigned char* meta, const T* qb, long long qst, const T* gb, long long gst,
                                                   const float* __restrict__ lse, const float* __restrict__ delta) {
   if (qp < npieces) {
-    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = qp % kStages, w = geo.w;
+    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = qp % kStages<HD>, w = geo.w;
     bool qv = false;
     long long tq = 0;
     int qa = 0, qb2 = 0, cut = 0;
@@ -690,6 +708,18 @@ __device__ __forceinline__ int query_epilogue(const Geo& geo) {
   return (geo.has_bias ? 3 : 0) + (geo.exact == 1 ? 1 : geo.exact == -1 ? 2 : 0);
 }
 
+// Dropout bits of query piece qp in pass 2: bit i = element i of the thread's fragment is kept
+__device__ __forceinline__ uint32_t query_piece_keep(const Geo& geo, const Visit* vl, const QueryCols& qc, int qp, int piece,
+                                                     int b, int h) {
+  const int vi = qp / geo.npc;
+  const uint32_t c0 = (uint32_t)(geo.g + vl[vi].oi * geo.w2 + piece * 64), sid = 2u * (uint32_t)(b * geo.H + h);
+  uint32_t keep = 0;
+#pragma unroll 1
+  for (int i = 0; i < 32; ++i)
+    keep |= (uint32_t)drop_keep(geo, (uint32_t)qc.tok[acc_col(i)], c0 + (uint32_t)acc_row(i), sid) << i;
+  return keep;
+}
+
 // P^T into s and dS^T into dp for one query piece
 template <bool RPE, int MASK>
 __device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const Geo& geo, const QueryCols& qc, const float* tab,
@@ -707,9 +737,9 @@ __device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const
 }
 
 // held to 4 / 3 CTAs per SM (HD <= 32 / 64) without dropout, 3 / 2 with it: left alone, ptxas takes more registers and
-// fits one less
+// fits one less.  HD 128: 2 with or without dropout, what the 2-stage ring fits.
 template <typename T, int HD, typename TO, bool DROP = false>
-__global__ void __launch_bounds__(kThreads, (HD <= 32 ? 4 : 3) - (DROP ? 1 : 0))
+__global__ void __launch_bounds__(kThreads, HD > 64 ? 2 : (HD <= 32 ? 4 : 3) - (DROP ? 1 : 0))
 wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse, const float* __restrict__ delta,
            const float* __restrict__ table) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
@@ -719,9 +749,9 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
   T* Ks = reinterpret_cast<T*>(smem_raw);
   T* Vs = Ks + TILE;
   T* ring = Vs + TILE;                                            // stage s: Q at ring + 2 s TILE, dO after it
-  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages * TILE);
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages<HD> * TILE);
   const int cols = (int)query_cols_bytes(DROP);
-  Visit* vl = reinterpret_cast<Visit*>(meta + kStages * cols);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kStages<HD> * cols);
   int* kpos = reinterpret_cast<int*>(vl + 9);
   float* tab = reinterpret_cast<float*>(kpos + 64);
   const int tw = 4 * geo.w - 1;
@@ -747,32 +777,27 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
 
   const int npieces = visit_list(geo, KR, KC, -1, vl) * geo.npc;
   const int epi = query_epilogue(geo);
-  SlotWalk wk(geo, slot);
+  std::conditional_t<(HD > 64), SlotWalkLean, SlotWalk> wk(geo, slot);
   // the (b, h) slices of q, dO, lse and delta are recomputed at each issue: kept live across the loop, they cost the
   // dropout kernel at HD 32 a spill
   __syncthreads();                                                // the visit list, kpos
 #pragma unroll
-  for (int p = 0; p < kStages - 1; ++p)                           // the first group also carries K and V
+  for (int p = 0; p < kStages<HD> - 1; ++p)                       // the first group also carries K and V
     issue_query_piece<T, HD, DROP>(geo, p, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
                                    row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
   for (int qp = 0; qp < npieces; ++qp) {
-    ring_wait();
-    issue_query_piece<T, HD, DROP>(geo, qp + kStages - 1, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
+    ring_wait<HD>();
+    issue_query_piece<T, HD, DROP>(geo, qp + kStages<HD> - 1, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
                                    row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
-    const int st = qp % kStages;
+    const int st = qp % kStages<HD>;
     const T* Qs = ring + st * 2 * TILE;
     const T* Gs = Qs + TILE;
     const QueryCols qcol = query_cols(meta, st, cols);
-    // dropout: bit i = element i is kept.  Drawn before the products: the draws need neither, and with s and dp not yet
-    // live the Philox rounds fit 3 CTAs per SM without spilling (HD <= 32).
+    // dropout: bit i = element i is kept.  Up to HD 64 drawn before the products: the draws need neither, and with s and
+    // dp not yet live the Philox rounds fit 3 CTAs per SM without spilling (HD <= 32).  At HD 128 drawn after them: held
+    // across the products, the bits and the walk cost the kernel a spill.
     uint32_t keep = 0;
-    if constexpr (DROP) {
-      const int vi = qp / geo.npc;
-      const uint32_t c0 = (uint32_t)(geo.g + vl[vi].oi * geo.w2 + cid.piece * 64), sid = 2u * (uint32_t)(b * geo.H + h);
-#pragma unroll 1
-      for (int i = 0; i < 32; ++i)
-        keep |= (uint32_t)drop_keep(geo, (uint32_t)qcol.tok[acc_col(i)], c0 + (uint32_t)acc_row(i), sid) << i;
-    }
+    if constexpr (DROP && HD <= 64) keep = query_piece_keep(geo, vl, qcol, qp, cid.piece, b, h);
     float s[32], dp[32];
     sm90::wg_fence();
 #pragma unroll
@@ -783,6 +808,7 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     sm90::wg_wait0();
     sm90::reg_fence(s);
     sm90::reg_fence(dp);
+    if constexpr (DROP && HD > 64) keep = query_piece_keep(geo, vl, qcol, qp, cid.piece, b, h);
     if constexpr (DROP) {    // dS = P (dP keep / (1 - p) - delta); the A operand of dV is P keep / (1 - p)
 #pragma unroll
       for (int i = 0; i < 32; ++i) dp[i] = (keep >> i) & 1u ? dp[i] * geo.drop_scale : 0.f;

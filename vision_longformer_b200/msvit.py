@@ -123,7 +123,7 @@ class DenseAttention(nn.Module):
     impl = "vil"  : the vil_attn sm_90a kernels - dense attention over nglo + w*w tokens is the SINGLE-CHUNK case of the
                     sliding-chunk operator (nx = ny = w, every local query sees every local key, global tokens as usual),
                     so the same tensor-core kernels serve it when w in {7, 14} (7x7 and 14x14 stages of the 224 nets),
-                    head dim <= 64, bf16/fp16 on CUDA; no (H,N,N) bias tensor is materialised: the Swin-style
+                    head dim <= 128 (a multiple of 8), bf16/fp16 on CUDA; no (H,N,N) bias tensor is materialised: the Swin-style
                     (2wx-1)(2wy-1) table is embedded in the operator's (4w-1)^2 index space (same Delta-row / Delta-col).
     impl = "sdpa" : stock F.scaled_dot_product_attention (cuDNN) with the bias as attn_mask.
     impl = "auto" : "sdpa": at 50..197 tokens the chunk-tiled kernels (64-row tiles, one global-token side kernel, two
@@ -175,7 +175,7 @@ class DenseAttention(nn.Module):
     def _vil_applies(self, x):
         w = self.wx
         return (self.impl == "vil" and x.is_cuda and self.wx == self.wy and w in (7, 14)
-                and x.shape[1] == self.nglo + w * w and (x.shape[2] // self.num_heads) <= 64
+                and x.shape[1] == self.nglo + w * w and (x.shape[2] // self.num_heads) <= 128
                 and (x.shape[2] // self.num_heads) % 8 == 0 and self.nglo <= 8
                 and (torch.is_autocast_enabled("cuda") or x.dtype in (torch.bfloat16, torch.float16)))
 
@@ -209,7 +209,7 @@ class DenseAttention(nn.Module):
                                       nglo=self.nglo, scale=self.scale, dropout_p=drop)
             return proj(out)
         if self.impl == "vil":
-            raise NotImplementedError("DenseAttention(impl='vil') needs a 7x7 or 14x14 token grid, head dim <= 64 and bf16/fp16 on CUDA")
+            raise NotImplementedError("DenseAttention(impl='vil') needs a 7x7 or 14x14 token grid, head dim <= 128 and bf16/fp16 on CUDA")
         q, k, v = _SplitQKV.apply(epilogue.linear_colsum_bias(x, self.qkv.weight, self.qkv.bias), self.num_heads)
         mask = self._bias(N).unsqueeze(0).to(q.dtype) if self.rpe else None
         out = F.scaled_dot_product_attention(q, k, v, attn_mask=mask,
