@@ -116,15 +116,19 @@ def _heads(t, H, which=0, parts=1):
     return t.view(B, T, parts, H, C // (parts * H))[:, :, which].permute(0, 2, 1, 3)
 
 
-def kernel_run(t, nx, ny, w, exact, mode, scale, dtype, impl, layout="contig", f32out=False, flags=0):
+def kernel_run(t, nx, ny, w, exact, mode, scale, dtype, impl, layout="contig", f32out=False, flags=0, drop=(0.0, 0, 0)):
     """One forward + backward through the C ABI.
     layout = "contig": contiguous (B,H,T,D) tensors;  "linear": the PRODUCTION layout - q / k / v are strided views of
     the `query` / `kv` Linear outputs ((B,N,H*D) with the global rows first, (B,N,2*H*D)), the output is head-merged
     (B,N,H*D), gradients are written into dq_all / dkv buffers of the same layouts (ops._heads; what bench.py and every
-    module call runs).  f32out: VIL_FLAG_F32_OUT parity build (bf16/fp16 inputs, fp32 outputs)."""
+    module call runs).  f32out: VIL_FLAG_F32_OUT parity build (bf16/fp16 inputs, fp32 outputs).
+    Separate global weights when t["kg"] / t["vg"] are not t["k"] / t["v"] (test_gpu_dropout.make_inputs): in the
+    linear layout they are views of a `kv_global` output, and their gradients come back as dkg / dvg.
+    drop = (p, seed, offset): attention dropout."""
     B, H, Nloc, D = t["q"].shape
     N = t["k"].shape[2]
     g = N - Nloc
+    sep = g > 0 and t.get("kg") is not None and t["kg"] is not t["k"]
     odt = torch.float32 if f32out else dtype
     f32 = lambda x: None if x is None else x.to(DEV, torch.float32).contiguous()
     table, g2l, g2g = f32(t["table"]), f32(t["g2l"]), f32(t["g2g"])
@@ -137,6 +141,10 @@ def kernel_run(t, nx, ny, w, exact, mode, scale, dtype, impl, layout="contig", f
         o, og = torch.empty_like(q, dtype=odt), (torch.empty_like(qg, dtype=odt) if g else None)
         dq, dk, dv = torch.empty_like(q, dtype=odt), torch.empty_like(k, dtype=odt), torch.empty_like(v, dtype=odt)
         dqg = torch.empty_like(qg, dtype=odt) if g else None
+        kg, vg, dkg, dvg = k, v, dk, dv
+        if sep:
+            kg, vg = dev(t["kg"]), dev(t["vg"])
+            dkg, dvg = torch.empty_like(kg, dtype=odt), torch.empty_like(vg, dtype=odt)
     else:
         C = H * D
         q_all = torch.empty(B, N, C, device=DEV, dtype=dtype)
@@ -154,17 +162,27 @@ def kernel_run(t, nx, ny, w, exact, mode, scale, dtype, impl, layout="contig", f
         o, og = _heads(out, H)[:, :, g:], (_heads(out, H)[:, :, :g] if g else None)
         dq, dqg = _heads(dq_all, H)[:, :, g:], (_heads(dq_all, H)[:, :, :g] if g else None)
         dk, dv = _heads(dkv, H, 0, 2), _heads(dkv, H, 1, 2)
-    kw = dict(nx=nx, ny=ny, w=w, exact=exact, mode=mode, scale=scale, impl=impl, flags=flags)
-    lse, lse_g = vil_attention_raw_forward(q, k, v, qg if g else None, k if g else None, v if g else None, table, g2l,
+        kg, vg, dkg, dvg = k, v, dk, dv
+        if sep:
+            kvg = torch.empty(B, N, 2 * C, device=DEV, dtype=dtype)
+            dkvg = torch.full((B, N, 2 * C), float("nan"), device=DEV, dtype=odt)
+            kg, vg = _heads(kvg, H, 0, 2), _heads(kvg, H, 1, 2)
+            kg.copy_(t["kg"]); vg.copy_(t["vg"])
+            dkg, dvg = _heads(dkvg, H, 0, 2), _heads(dkvg, H, 1, 2)
+    kw = dict(nx=nx, ny=ny, w=w, exact=exact, mode=mode, scale=scale, impl=impl, flags=flags,
+              dropout_p=drop[0], dropout_seed=drop[1], dropout_offset=drop[2])
+    lse, lse_g = vil_attention_raw_forward(q, k, v, qg if g else None, kg if g else None, vg if g else None, table, g2l,
                                            g2g, o, og, **kw)
     fam_f = _lib.last_impl()
     zl = lambda x: None if x is None else torch.zeros_like(x)
     dt, dgl, dgg = zl(table), zl(g2l), zl(g2g)
-    vil_attention_raw_backward(q, k, v, qg if g else None, k if g else None, v if g else None, table, g2l, g2g, o, og,
+    vil_attention_raw_backward(q, k, v, qg if g else None, kg if g else None, vg if g else None, table, g2l, g2g, o, og,
                                lse, lse_g, go, gog if g else None, dq, dk, dv, dqg,
-                               dk if g else None, dv if g else None, dt, dgl, dgg, **kw)
+                               dkg if g else None, dvg if g else None, dt, dgl, dgg, **kw)
     torch.cuda.synchronize()
     out_d = dict(o=o, og=og, lse=lse, lse_g=lse_g, dq=dq, dk=dk, dv=dv, dqg=dqg, dtable=dt, dg2l=dgl, dg2g=dgg)
+    if sep:
+        out_d.update(dkg=dkg, dvg=dvg)
     return out_d, fam_f, _lib.last_impl()
 
 
