@@ -223,6 +223,9 @@ int vil_layernorm_bwd_sm100(const VilLayerNormParams* p, void* stream);
  * vil_addnorm_bwd_sm100:  dx = gres + LayerNorm'(dy)  (x = the residual stream the norm saw, i.e. the forward's xo);
  *                         dbr = rowscale * dx;  dgamma, dbeta, dbias = column sums (deterministic two-stage reduction)
  * The residual stream (x, xo, gres, dx) is fp32; br / dbr carry b_dtype, y / dy carry y_dtype.  C % 4 == 0, C <= 1024.
+ * Contiguous tensors; every non-NULL pointer of a call must be 16-byte aligned (the kernels make 128-bit accesses to the
+ * fp32 rows and gamma, 64-bit ones to the bf16 / fp16 rows), else VIL_E_BADARG.  Caching-allocator tensors always are;
+ * a contiguous view that starts mid-allocation may not be.
  */
 typedef struct VilAddNormParams {
   int32_t struct_bytes;    /* = sizeof(VilAddNormParams) */

@@ -152,6 +152,15 @@ def launch_count() -> int:
     return int(load().vil_attn_launch_count())
 
 
+def aligned(t):
+    """`t` itself when its data starts on a 16-byte boundary (every caching-allocator tensor does), else an aligned copy.
+    The epilogue kernels make 128-bit accesses and the library refuses misaligned pointers; a contiguous view can still
+    start at any element (`buf[1:].view(...)`, a parameter that is a view into a flat buffer)."""
+    if t is None or t.data_ptr() % 16 == 0:
+        return t
+    return t.clone()                     # callers pass contiguous tensors: the fresh copy keeps their strides
+
+
 def raise_for(code: int):
     """Map a C return code to the exception type the reference raises for the same condition
     (asserts / ValueError in longformer2d.py:111, slidingchunk_2d.py:343)."""

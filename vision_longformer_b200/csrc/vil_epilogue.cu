@@ -30,6 +30,15 @@ int an_check(const VilAddNormParams* p, bool bwd) {
   if (p->rows == 0) return VIL_OK;                  // empty stream: nothing is read or launched (empty tensors have NULL data)
   if (p->br != nullptr && p->b_dtype != p->y_dtype && p->b_dtype != VIL_F32 && p->y_dtype != VIL_F32)
     return efail(VIL_E_UNSUPPORTED, "addnorm: br and y must share their low-precision type");
+  // 128-bit accesses to the fp32 rows and gamma, 64-bit ones to the low-precision rows: one rule for every pointer of the call
+  // (checked before the NULL checks, so that a refused call never depends on which other tensors were given)
+  const uintptr_t al = !bwd
+      ? ((uintptr_t)p->x | (uintptr_t)p->br | (uintptr_t)p->bias | (uintptr_t)p->rowscale | (uintptr_t)p->gamma |
+         (uintptr_t)p->beta | (uintptr_t)p->xo | (uintptr_t)p->y | (uintptr_t)p->mean | (uintptr_t)p->rstd)
+      : ((uintptr_t)p->x | (uintptr_t)p->gamma | (uintptr_t)p->beta | (uintptr_t)p->rowscale | (uintptr_t)p->mean |
+         (uintptr_t)p->rstd | (uintptr_t)p->dy | (uintptr_t)p->gres | (uintptr_t)p->dx | (uintptr_t)p->dbr |
+         (uintptr_t)p->dgamma | (uintptr_t)p->dbeta | (uintptr_t)p->dbias | (uintptr_t)p->workspace);
+  if (al & 15) return efail(VIL_E_BADARG, "addnorm: tensors must be 16-byte aligned");
   if (!p->x || !p->gamma || !p->beta || !p->mean || !p->rstd) return efail(VIL_E_BADARG, "addnorm: NULL tensor");
   if (p->rowscale != nullptr && p->rows_per_sample <= 0) return efail(VIL_E_BADARG, "addnorm: rows_per_sample must be positive");
   if (!bwd) {

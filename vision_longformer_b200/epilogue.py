@@ -13,6 +13,7 @@ oracle attention for the reference arm).
 from __future__ import annotations
 
 import ctypes
+import math
 
 import torch
 import torch.nn.functional as F
@@ -20,6 +21,7 @@ import torch.nn.functional as F
 from . import _lib
 
 _DT = {torch.float32: _lib.VIL_F32, torch.bfloat16: _lib.VIL_BF16, torch.float16: _lib.VIL_F16}
+_aligned = _lib.aligned
 
 
 def _stream(t):
@@ -75,11 +77,11 @@ class _AddNorm(torch.autograd.Function):
     @torch.amp.custom_fwd(device_type="cuda")
     def forward(ctx, x, br, bias, rowscale, gamma, beta, eps, out_dtype, rows_per_sample):
         C = x.shape[-1]
-        x2 = x.reshape(-1, C).contiguous()
-        br2 = br.reshape(-1, C).contiguous()
-        g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
-        bias32 = None if bias is None else bias.detach().float().contiguous()
-        rs32 = None if rowscale is None else rowscale.detach().float().contiguous()
+        x2 = _aligned(x.reshape(-1, C).contiguous())
+        br2 = _aligned(br.reshape(-1, C).contiguous())
+        g32, b32 = _aligned(gamma.detach().float().contiguous()), _aligned(beta.detach().float().contiguous())
+        bias32 = None if bias is None else _aligned(bias.detach().float().contiguous())
+        rs32 = None if rowscale is None else _aligned(rowscale.detach().float().contiguous())
         rows = x2.shape[0]
         xo = torch.empty_like(x2)
         y = torch.empty((rows, C), dtype=out_dtype, device=x.device)
@@ -101,11 +103,11 @@ class _AddNorm(torch.autograd.Function):
         if g_y is None:
             g_y = torch.zeros((rows, C), dtype=out_dtype, device=dev)
         dy = g_y.reshape(-1, C)
-        dy = (dy if dy.dtype == out_dtype else dy.to(out_dtype)).contiguous()
+        dy = _aligned((dy if dy.dtype == out_dtype else dy.to(out_dtype)).contiguous())
         gres = None
         if g_xo is not None:
             gres = g_xo.reshape(-1, C)
-            gres = (gres if gres.dtype == torch.float32 else gres.float()).contiguous()
+            gres = _aligned((gres if gres.dtype == torch.float32 else gres.float()).contiguous())
         dx = torch.empty_like(xo)
         dbr = torch.empty((rows, C), dtype=br_dtype, device=dev)
         alloc = torch.zeros if rows == 0 else torch.empty
@@ -116,10 +118,14 @@ class _AddNorm(torch.autograd.Function):
 
 
 def add_norm(x, br, bias, rowscale, norm, out_dtype=None):
-    """xo = x + rowscale[sample] * (br + bias);  y = norm(xo).  `norm`: an affine last-dim nn.LayerNorm.  x: (B, N, C) fp32."""
+    """xo = x + rowscale[sample] * (br + bias);  y = norm(xo).  `norm`: an affine last-dim nn.LayerNorm.  x: (B, ..., C) fp32;
+    rowscale: (B) with one entry per sample x[b], or None."""
     if out_dtype is None:
         out_dtype = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else x.dtype
-    rps = x.shape[1] if x.dim() == 3 else 1
+    if rowscale is not None and (x.dim() < 2 or rowscale.numel() != x.shape[0]):
+        raise ValueError(f"add_norm: rowscale has {rowscale.numel()} entries for a stream of shape {tuple(x.shape)}; "
+                         "it needs one per sample (x.shape[0])")
+    rps = math.prod(x.shape[1:-1])                         # rows of one sample: every dim between the batch and the channels
     return _AddNorm.apply(x, br, bias, rowscale, norm.weight, norm.bias, norm.eps, out_dtype, rps)
 
 
@@ -169,8 +175,8 @@ class _BiasGelu(torch.autograd.Function):
     @torch.amp.custom_fwd(device_type="cuda")
     def forward(ctx, z, bias):
         C = z.shape[-1]
-        z2 = z.reshape(-1, C).contiguous()
-        b32 = bias.detach().float().contiguous()
+        z2 = _aligned(z.reshape(-1, C).contiguous())
+        b32 = _aligned(bias.detach().float().contiguous())
         a = torch.empty_like(z2)
         bias_act_raw_forward(z2, b32, a, _lib.VIL_ACT_GELU)
         ctx.save_for_backward(z2, b32)
@@ -183,7 +189,7 @@ class _BiasGelu(torch.autograd.Function):
         z2, b32 = ctx.saved_tensors
         shape, bdt = ctx.meta
         da2 = da.reshape(-1, z2.shape[1])
-        da2 = (da2 if da2.dtype == z2.dtype else da2.to(z2.dtype)).contiguous()
+        da2 = _aligned((da2 if da2.dtype == z2.dtype else da2.to(z2.dtype)).contiguous())
         dz, dbias = _colsum(da2, z2, b32, _lib.VIL_ACT_GELU)
         return dz.view(shape), dbias.to(bdt)
 
@@ -208,7 +214,7 @@ class _LinearColsumBias(torch.autograd.Function):
     def backward(ctx, dy):
         x, weight = ctx.saved_tensors
         Cout, Cin = weight.shape
-        dy2 = dy.reshape(-1, Cout).contiguous()
+        dy2 = _aligned(dy.reshape(-1, Cout).contiguous())
         dx = dw = None
         if ctx.needs_input_grad[0]:
             dx = (dy2 @ weight).view(x.shape)

@@ -38,9 +38,8 @@ class _FusedLayerNorm(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, eps, out_dtype):
         C = x.shape[-1]
-        x2 = x.reshape(-1, C)
-        x2 = x2 if x2.is_contiguous() else x2.contiguous()
-        w32, b32 = weight.detach().float().contiguous(), bias.detach().float().contiguous()
+        x2 = _lib.aligned(x.reshape(-1, C).contiguous())
+        w32, b32 = _lib.aligned(weight.detach().float().contiguous()), _lib.aligned(bias.detach().float().contiguous())
         y = torch.empty(x2.shape, dtype=out_dtype, device=x.device)
         mean = torch.empty(x2.shape[0], dtype=torch.float32, device=x.device)
         rstd = torch.empty_like(mean)
@@ -63,7 +62,7 @@ class _FusedLayerNorm(torch.autograd.Function):
         dy2 = dy.reshape(-1, C)
         if dy2.dtype != out_dtype:
             dy2 = dy2.to(out_dtype)
-        dy2 = dy2 if dy2.is_contiguous() else dy2.contiguous()
+        dy2 = _lib.aligned(dy2.contiguous())
         dx = torch.empty_like(x2)
         # rows == 0: the library returns without launching, so the parameter gradients must already be zero
         alloc = torch.zeros if x2.shape[0] == 0 else torch.empty
