@@ -12,7 +12,8 @@ Metrics (all against the fp64 dense oracle on the inputs rounded to the kernel's
                                   from local ones; the failure message names the row's chunk, 64-row piece and edge state
   per chunk                       max over (image, head, chunk) of the norm-relative error of the chunk's block
   lse, lse_g                      max absolute error, finite everywhere
-  bias gradients                  whole-tensor norm (they are sums over everything), at the bars of test_gpu_parity
+  bias gradients                  whole-tensor norm at the bars of test_gpu_parity; tests/test_gpu_bias_entries.py holds
+                                  them entry by entry
 The floor is 0 except under a saturated softmax (`peak_floors`).  Every maximum is recorded (tests.util.record).
 
 The bars were measured on an H100 SXM (700 W power limit): each is at most about 3x the worst value seen over this file
