@@ -55,8 +55,8 @@ enum { VIL_F32 = 0, VIL_BF16 = 1, VIL_F16 = 2 };
 /* kernel family selection */
 enum {
   VIL_IMPL_AUTO    = 0, /* wgmma path when the configuration is covered, else SIMT */
-  VIL_IMPL_SIMT    = 1, /* CUDA-core fp32 path: every (w, exact, mode, nglo) incl. fp32 I/O; forward D <= 128,
-                           backward and dropout D <= 64 */
+  VIL_IMPL_SIMT    = 1, /* CUDA-core fp32 path: every (w, exact, mode, nglo) incl. fp32 I/O; forward D <= 128;
+                           backward and dropout D <= 128 in fp32, D <= 64 in bf16 / fp16 */
   VIL_IMPL_WGMMA   = 2  /* wgmma tensor-core path (bf16/fp16, D <= 128 with D % 8 == 0 and 16-byte-aligned rows; with
                            the bias table w <= 42 when D > 64): error if the configuration is not covered */
 };

@@ -151,13 +151,14 @@ __device__ __forceinline__ void drop_keep2(const Geo& g, uint32_t row, uint32_t 
 // (dR, dC); masked pairs, rows past the chunk and empty slots hold 0.  The pair (query qr, qc; key kr, kc) adds to entry
 // (qr - kr - dR w + 2w - 1) (4w - 1) + (qc - kc - dC w + 2w - 1).  The pairs of one entry have one (u, v) = (qr - kr,
 // qc - kc), so its queries form a rectangle, clipped to the two pieces' slot ranges row by row.  The (2w - 1)^2 windows
-// (u, v) are dealt out to the 128 threads; each adds its pairs in ascending query-slot order and then adds that sum to
-// acc[entry], which no other thread touches until the next barrier.  Every CTA thereby sums in one fixed order.
+// (u, v) are dealt out to the `nthreads` threads of the CTA; each adds its pairs in ascending query-slot order and then
+// adds that sum to acc[entry], which no other thread touches until the next barrier.  Every CTA thereby sums in one fixed
+// order, whatever the number of threads that share the windows.
 __device__ __forceinline__ void table_grad_piece(const float* tile, int ld, float* acc, const Geo& geo, int dR, int dC,
-                                                 int qp, int kp) {
+                                                 int qp, int kp, int nthreads = 128) {
   const int w = geo.w, tw = 4 * w - 1, ww = 2 * w - 1;
   const int q0 = qp * 64, k0 = kp * 64;
-  for (int x = threadIdx.x; x < ww * ww; x += 128) {
+  for (int x = threadIdx.x; x < ww * ww; x += nthreads) {
     const int u = x / ww - (w - 1), v = x % ww - (w - 1);
     const int c_lo = max(0, v), c_hi = min(w - 1, w - 1 + v);
     float sum = 0.f;
