@@ -1,8 +1,9 @@
-"""fp32 training at head dims 64 < D <= 128 on the SIMT family: the four-lanes-per-row kernels (vil_simt.cuh, Tile4).
+"""fp32 training at head dims 64 < D <= 128 on the SIMT family: the local kernels at four lanes per row (vil_simt.cuh,
+L = 4, Tile<128, 4>).
 
-The fp32 backward at D > 64 and the fp32 dropout forward at D > 64 run simt_bwd_dq4 / simt_bwd_dkv4 / simt_fwd_local4;
-the forward without dropout stays on the two-lane kernel.  Everything is held with the machinery of the other files, at
-their SIMT fp32 bars:
+The fp32 backward at D > 64 and the fp32 dropout forward at D > 64 run simt_bwd_dq<float, 128, 4, DROP, TAB> /
+simt_bwd_dkv<float, 128, 4, DROP> / simt_fwd_local<float, 128, 4, true>; the forward without dropout stays on the
+two-lane kernel.  Everything is held with the machinery of the other files, at their SIMT fp32 bars:
   rows and chunks of every output against the fp64 dense oracle     test_gpu_attention_rows (check, oracle)
   the bias gradients entry by entry                                  test_gpu_bias_entries (hold_entries)
   dropout against the exact-mask restatement                         test_gpu_dropout (reference_run)

@@ -155,7 +155,7 @@ __device__ __forceinline__ void drop_keep2(const Geo& g, uint32_t row, uint32_t 
 // adds that sum to acc[entry], which no other thread touches until the next barrier.  Every CTA thereby sums in one fixed
 // order, whatever the number of threads that share the windows.
 __device__ __forceinline__ void table_grad_piece(const float* tile, int ld, float* acc, const Geo& geo, int dR, int dC,
-                                                 int qp, int kp, int nthreads = 128) {
+                                                 int qp, int kp, int nthreads) {
   const int w = geo.w, tw = 4 * w - 1, ww = 2 * w - 1;
   const int q0 = qp * 64, k0 = kp * 64;
   for (int x = threadIdx.x; x < ww * ww; x += nthreads) {

@@ -9,7 +9,7 @@ namespace {
 
 int head_bucket(int D) { return D <= 8 ? 8 : D <= 16 ? 16 : D <= 32 ? 32 : D <= 64 ? 64 : 128; }
 
-// HS: floats per tile row (Tile<HD>::HS, Tile4<HD>::HS)
+// HS: floats per tile row (Tile<HD, L>::HS)
 size_t simt_tile_smem(const Geo& g, int HS, bool dkv) {
   const int tw = 4 * g.w - 1;
   size_t bytes = (size_t)(2 * 64 * HS + (g.has_bias ? tw * tw : 0)) * sizeof(float);
@@ -80,23 +80,22 @@ int global_bwd_t(const VilAttnParams* p, const Geo& g, cudaStream_t s, int rmw_r
   HDM(__half, __half, CALL)
 
 // ------------------------------------------------------------------ SIMT family proper
-// fp32 backward and dropout at 64 < D <= 128 run the four-lanes-per-row kernels (vil_simt.cuh: two lanes per row would
-// spill); bf16 / fp16 train at those head dims on the wgmma family
-template <typename T, int HD> constexpr bool kQuadRows = HD > 64 && std::is_same<T, float>::value;
-
+// L: lanes per row of the local-query kernels (vil_simt.cuh).  fp32 backward and dropout at 64 < D <= 128 run four (two
+// would spill); the forward without dropout runs two at every head dim.  bf16 / fp16 train at those head dims on the
+// wgmma family.
 template <typename T, int HD, bool DROP>
 int simt_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
-  if constexpr (DROP && HD > 64 && !kQuadRows<T, HD>) {   // the bf16 / fp16 backward stops at 64 as well
+  if constexpr (DROP && HD > 64 && !std::is_same<T, float>::value) {   // the bf16 / fp16 backward stops at 64 as well
     return shared_fail(VIL_E_UNSUPPORTED, "attention dropout supports head dim <= 64");
   } else {
-  constexpr bool quad = DROP && kQuadRows<T, HD>;          // without dropout the two-lane kernel serves every head dim
-  const auto kernel = [] { if constexpr (quad) return simt_fwd_local4<T, HD, DROP>; else return simt_fwd_local<T, HD, DROP>; }();
-  const size_t sm = simt_tile_smem(g, quad ? Tile4<HD>::HS : Tile<HD>::HS, false);
+  constexpr int L = DROP && std::is_same<T, float>::value && HD > 64 ? 4 : 2;
+  const auto kernel = simt_fwd_local<T, HD, L, DROP>;
+  const size_t sm = simt_tile_smem(g, Tile<HD, L>::HS, false);
   int rc = set_smem(kernel, sm);
   if (rc) return rc;
   const long long blocks = (long long)g.B * g.H * g.mx * g.my * g.npc;
   if (!(p->skip_mask & 2)) {
-    kernel<<<(unsigned)blocks, quad ? 256 : 128, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse, p->bias_table, p->g2l);
+    kernel<<<(unsigned)blocks, 64 * L, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse, p->bias_table, p->g2l);
     count_launch();
   }
   if (g.g > 0 && !(p->skip_mask & 1)) {
@@ -107,41 +106,39 @@ int simt_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
 }
 
 // backward pass 1; TAB (the bias table): nslice image slices per (head, chunk, piece), table partials into the workspace
-template <typename T, int HD, bool DROP, bool TAB>
+template <typename T, int HD, int L, bool DROP, bool TAB>
 int simt_dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
-  constexpr bool quad = kQuadRows<T, HD>;
-  const auto kernel = [] { if constexpr (quad) return simt_bwd_dq4<T, HD, DROP, TAB>; else return simt_bwd_dq<T, HD, DROP, TAB>; }();
-  const size_t sm = simt_tile_smem(g, quad ? Tile4<HD>::HS : Tile<HD>::HS, false) + (TAB ? simt_ds_tile_bytes() : 0);
+  const auto kernel = simt_bwd_dq<T, HD, L, DROP, TAB>;
+  const size_t sm = simt_tile_smem(g, Tile<HD, L>::HS, false) + (TAB ? simt_ds_tile_bytes() : 0);
   int rc = set_smem(kernel, sm);
   if (rc) return rc;
   const long long ctas = TAB ? tab_ctas(g) : (long long)g.B * g.H * g.mx * g.my * g.npc;
-  kernel<<<(unsigned)ctas, quad ? 256 : 128, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse,
-                                                      ws_delta(p), p->bias_table, p->g2l,
-                                                      TAB ? ws_at(p, ws_off_tab(g)) : nullptr);
+  kernel<<<(unsigned)ctas, 64 * L, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse, ws_delta(p),
+                                            p->bias_table, p->g2l, TAB ? ws_at(p, ws_off_tab(g)) : nullptr);
   count_launch();
   return VIL_OK;
 }
 
 template <typename T, int HD, bool DROP>
 int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
-  if constexpr (HD > 64 && !kQuadRows<T, HD>) {
+  if constexpr (HD > 64 && !std::is_same<T, float>::value) {
     return shared_fail(VIL_E_UNSUPPORTED,
                        "the SIMT backward supports head dim <= 64; 64 < D <= 128 is trained by the wgmma family "
                        "(bf16 / fp16 with 16-byte-aligned rows)");
   } else {
-    constexpr bool quad = kQuadRows<T, HD>;
+    constexpr int L = std::is_same<T, float>::value && HD > 64 ? 4 : 2;
     int rc = (p->skip_mask & 8) ? VIL_OK : delta_t<T, T>(p, g, s);
     if (rc) return rc;
-    const auto dkv = [] { if constexpr (quad) return simt_bwd_dkv4<T, HD, DROP>; else return simt_bwd_dkv<T, HD, DROP>; }();
-    const size_t sm2 = simt_tile_smem(g, quad ? Tile4<HD>::HS : Tile<HD>::HS, true);
+    const auto dkv = simt_bwd_dkv<T, HD, L, DROP>;
+    const size_t sm2 = simt_tile_smem(g, Tile<HD, L>::HS, true);
     if ((rc = set_smem(dkv, sm2))) return rc;
     const long long blocks = (long long)g.B * g.H * g.mx * g.my * g.npc;
     if (!(p->skip_mask & 2)) {
-      if ((rc = g.has_bias ? simt_dq_pass<T, HD, DROP, true>(p, g, s) : simt_dq_pass<T, HD, DROP, false>(p, g, s))) return rc;
+      if ((rc = g.has_bias ? simt_dq_pass<T, HD, L, DROP, true>(p, g, s) : simt_dq_pass<T, HD, L, DROP, false>(p, g, s))) return rc;
     }
     if (!(p->skip_mask & 4)) {
-      dkv<<<(unsigned)blocks, quad ? 256 : 128, sm2, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv),
-                                                          p->lse, ws_delta(p), p->bias_table);
+      dkv<<<(unsigned)blocks, 64 * L, sm2, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv), p->lse,
+                                                ws_delta(p), p->bias_table);
       count_launch();
     }
     if (g.g > 0 && !(p->skip_mask & 1)) {

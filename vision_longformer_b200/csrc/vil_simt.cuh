@@ -2,7 +2,7 @@
 //
 // Covers EVERY configuration of the reference operator (any w, exact in {0,1,-1},
 // mode in {-1,0,1..8}, any nglo, fp32 / bf16 / fp16 I/O) at D <= 128, with one limit: backward
-// and dropout at 64 < D <= 128 are fp32 only (the four-lanes-per-row kernels below); bf16 / fp16
+// and dropout at 64 < D <= 128 are fp32 only (the local kernels at four lanes per row); bf16 / fp16
 // SIMT training stops at D = 64.  It is (a) the fp32 parity build (1e-5 vs the fp64 oracle),
 // (b) the path for configurations the wgmma family does not cover, and (c) the home of
 // the small global-token kernels that both families share (every D <= 128: bf16 / fp16
@@ -22,12 +22,25 @@
 
 namespace vil {
 
-// fp32 smem tile row: two halves of HD/2 floats separated by 4 floats of padding so that the two
-// threads of a (row, half) pair hit different banks.
-template <int HD> struct Tile {
-  static constexpr int HH = HD / 2;
-  static constexpr int HS = HD + 8;
-  static __device__ __forceinline__ int off(int half) { return half * (HH + 4); }
+// ----------------------------------------------------------------------------------------------
+// Local-query kernels: CTA = one 64-slot piece of one chunk of one (b,h), L lanes per row.  Lane `part` = tid & (L-1) of
+// slot tid >> (L/2) owns the HP = HD/L consecutive channels [part HP, part HP + HP) of its row; a dot product is its
+// HP-term FMA chain plus log2(L) xor-shuffle steps, and lane 0 of a slot writes the per-row values (lse, delta, the dS
+// tile, the staged key / query metadata).  L = 2, except for fp32 training at 64 < D <= 128: at HD 128 two lanes would
+// hold 64 floats per row tensor (192 in pass 1, 256 in pass 2) and spill, so those kernels run L = 4.  The grids, the
+// workspace and the fixed order of the table gradient do not depend on L.  The lane decode is a shift and a mask (tid is
+// signed: tid / L, tid % L compile to different code), and the shuffle steps and the key-piece staging of the forward
+// and pass 1 are written out in each kernel: moved into __forceinline__ helpers (group_sum<L> included), they compile
+// to differently scheduled SASS.
+// ----------------------------------------------------------------------------------------------
+// fp32 smem tile row: L parts of HP floats.  L = 2: the halves are 4 floats apart, so the two threads of a (row, half)
+// pair hit different banks.  L = 4: the quarters sit at a stride of HP + 1, so the four lanes of a row hit four banks and
+// the 8 rows a warp stages hit all 32 (the row stride HD + 4 is 4 banks); with the HD + 8 row, pass 1 with the table at
+// HD 128 and w = 48 would need 232 528 bytes, 80 over the limit, and with HD + 4 it needs 230 480.
+template <int HD, int L> struct Tile {
+  static constexpr int HP = HD / L;
+  static constexpr int HS = L == 2 ? HD + 8 : HD + 4;
+  static __device__ __forceinline__ int off(int part) { return part * (HP + (L == 2 ? 4 : 1)); }
 };
 
 struct ChunkId { int b, h, R, C, piece; };
@@ -43,15 +56,14 @@ __device__ __forceinline__ ChunkId decode_block(const Geo& g, int bid) {
 }
 
 // ----------------------------------------------------------------------------------------------
-// forward, local queries.  CTA = one 64-query piece of one chunk of one (b,h); thread pair per query,
-// each thread owns half of the head dimension.
+// forward, local queries
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, bool DROP = false>
-__global__ void __launch_bounds__(128)
+template <typename T, int HD, int L, bool DROP>
+__global__ void __launch_bounds__(64 * L, L == 4 ? 1 : 0)
 simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
                const float* __restrict__ table, const float* __restrict__ g2l) {
-  using TL = Tile<HD>;
-  constexpr int HH = TL::HH, HS = TL::HS;
+  using TL = Tile<HD, L>;
+  constexpr int HP = TL::HP, HS = TL::HS;
   extern __shared__ float smem[];
   float* Ks = smem;
   float* Vs = Ks + 64 * HS;
@@ -64,20 +76,20 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
-  const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
+  const int tid = threadIdx.x, slot = tid >> (L / 2), part = tid & (L - 1);
   const int w = geo.w, D = geo.D;
 
-  for (int i = tid; i < tabn; i += 128) tab[i] = table[(long long)i * geo.H + h];
+  for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
 
   const int l = cid.piece * 64 + slot;
   const int qr = l / w, qc = l % w;
   const int r = R * w + qr, c = C * w + qc;
   const bool qvalid = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
 
-  float qh[HH], oh[HH];
+  float qh[HP], oh[HP];
 #pragma unroll
-  for (int i = 0; i < HH; ++i) { qh[i] = 0.f; oh[i] = 0.f; }
-  if (qvalid) load_seg<T, HH>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), half * HH, D, qh);
+  for (int i = 0; i < HP; ++i) { qh[i] = 0.f; oh[i] = 0.f; }
+  if (qvalid) load_seg<T, HP>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), part * HP, D, qh);
   float m = -INFINITY, lsum = 0.f;
   const uint32_t drow = (uint32_t)(r * geo.ny + c), dsid = 2u * (uint32_t)(b * geo.H + h);   // dropout: row, stream 0
 
@@ -97,10 +109,10 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
       else if (KR < 0 || KR >= geo.mx || KC < 0 || KC >= geo.my) continue;   // CTA-uniform
     }
     __syncthreads();
-    {   // stage one piece of <=64 keys: thread pair (slot, half) loads half a row of K and V
-      float kk[HH], vv[HH];
+    {   // stage one piece of <=64 keys: lane `part` of a slot loads its HP channels of a row of K and V
+      float kk[HP], vv[HP];
 #pragma unroll
-      for (int i = 0; i < HH; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
+      for (int i = 0; i < HP; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
       int flag = 0, vr = 0, vc = 0; long long tok = -1;
       if (isg) {
         const int t = pi * 64 + slot;
@@ -121,24 +133,25 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
         }
       }
       if (tok >= 0) {
-        load_seg<T, HH>(row_ptr<T>(k, b, h, tok), half * HH, D, kk);
-        load_seg<T, HH>(row_ptr<T>(v, b, h, tok), half * HH, D, vv);
+        load_seg<T, HP>(row_ptr<T>(k, b, h, tok), part * HP, D, kk);
+        load_seg<T, HP>(row_ptr<T>(v, b, h, tok), part * HP, D, vv);
       }
-      float* kd = Ks + slot * HS + TL::off(half);
-      float* vd = Vs + slot * HS + TL::off(half);
+      float* kd = Ks + slot * HS + TL::off(part);
+      float* vd = Vs + slot * HS + TL::off(part);
 #pragma unroll
-      for (int i = 0; i < HH; ++i) { kd[i] = kk[i]; vd[i] = vv[i]; }
-      if (half == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
+      for (int i = 0; i < HP; ++i) { kd[i] = kk[i]; vd[i] = vv[i]; }
+      if (part == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
     }
     __syncthreads();
     for (int j = 0; j < 64; ++j) {
       const int f = kfl[j];
       if (!f) continue;                                   // warp-uniform
-      const float* kd = Ks + j * HS + TL::off(half);
+      const float* kd = Ks + j * HS + TL::off(part);
       float sp = 0.f;
 #pragma unroll
-      for (int i = 0; i < HH; ++i) sp = fmaf(qh[i], kd[i], sp);
-      sp += __shfl_xor_sync(0xffffffffu, sp, 1);
+      for (int i = 0; i < HP; ++i) sp = fmaf(qh[i], kd[i], sp);
+      sp += __shfl_xor_sync(0xffffffffu, sp, 1);           // over the L lanes of the row
+      if constexpr (L == 4) sp += __shfl_xor_sync(0xffffffffu, sp, 2);
       float bias = 0.f; bool ok = qvalid;
       if (f == 2) {
         if (geo.has_bias) bias = g2l[((long long)geo.H + h) * geo.g + kvr[j]];
@@ -149,34 +162,20 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
       }
       if (ok) {
         const float s = fmaf(geo.scale, sp, bias);
-        const float* vd = Vs + j * HS + TL::off(half);
-        if constexpr (DROP) {            // lsum sums the undropped P; O sums P * keep, scaled by 1 / (1 - p) at the end
-          const float km = drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? 1.f : 0.f;
-          if (s > m) {
-            const float corr = __expf(m - s);
-            lsum = lsum * corr + 1.f;
+        const float* vd = Vs + j * HS + TL::off(part);
+        // dropout: lsum sums the undropped P; O sums P * keep, scaled by 1 / (1 - p) at the end
+        const float km = DROP ? (drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? 1.f : 0.f) : 1.f;
+        if (s > m) {
+          const float corr = __expf(m - s);
+          lsum = lsum * corr + 1.f;
 #pragma unroll
-            for (int i = 0; i < HH; ++i) oh[i] = fmaf(oh[i], corr, km * vd[i]);
-            m = s;
-          } else {
-            const float p = __expf(s - m);
-            lsum += p;
-#pragma unroll
-            for (int i = 0; i < HH; ++i) oh[i] = fmaf(p * km, vd[i], oh[i]);
-          }
+          for (int i = 0; i < HP; ++i) oh[i] = fmaf(oh[i], corr, km * vd[i]);
+          m = s;
         } else {
-          if (s > m) {
-            const float corr = __expf(m - s);
-            lsum = lsum * corr + 1.f;
+          const float p = __expf(s - m);
+          lsum += p;
 #pragma unroll
-            for (int i = 0; i < HH; ++i) oh[i] = fmaf(oh[i], corr, vd[i]);
-            m = s;
-          } else {
-            const float p = __expf(s - m);
-            lsum += p;
-#pragma unroll
-            for (int i = 0; i < HH; ++i) oh[i] = fmaf(p, vd[i], oh[i]);
-          }
+          for (int i = 0; i < HP; ++i) oh[i] = fmaf(p * km, vd[i], oh[i]);
         }
       }
     }
@@ -184,10 +183,10 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
   if (qvalid) {
     const float inv = (lsum > 0.f ? 1.f / lsum : 0.f) * (DROP ? geo.drop_scale : 1.f);
 #pragma unroll
-    for (int i = 0; i < HH; ++i) oh[i] *= inv;
+    for (int i = 0; i < HP; ++i) oh[i] *= inv;
     const long long tokq = (long long)r * geo.ny + c;
-    store_seg<T, HH>(row_ptr_w<T>(o, b, h, tokq), half * HH, D, oh);
-    if (half == 0) lse[((long long)b * geo.H + h) * geo.Nloc + tokq] = m + logf(lsum);
+    store_seg<T, HP>(row_ptr_w<T>(o, b, h, tokq), part * HP, D, oh);
+    if (part == 0) lse[((long long)b * geo.H + h) * geo.Nloc + tokq] = m + logf(lsum);
   }
 }
 
@@ -330,13 +329,13 @@ __global__ void simt_bwd_delta(Geo geo, T4 o, T4 d_o, T4 og, T4 d_og,
 constexpr int kSimtDsLd = 65;   // dS tile row stride: the 16 query slots of a warp write one column in distinct banks
 inline size_t simt_ds_tile_bytes() { return 64 * kSimtDsLd * sizeof(float); }
 
-template <typename T, int HD, bool DROP = false, bool TAB = false>
-__global__ void __launch_bounds__(128, TAB && HD <= 8 ? 4 : 0)
+template <typename T, int HD, int L, bool DROP, bool TAB>
+__global__ void __launch_bounds__(64 * L, L == 4 ? 1 : (TAB && HD <= 8 ? 4 : 0))
 simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse,
             const float* __restrict__ delta, const float* __restrict__ table,
             const float* __restrict__ g2l, float* __restrict__ tpart) {
-  using TL = Tile<HD>;
-  constexpr int HH = TL::HH, HS = TL::HS;
+  using TL = Tile<HD, L>;
+  constexpr int HP = TL::HP, HS = TL::HS;
   extern __shared__ float smem[];
   float* Ks = smem;
   float* Vs = Ks + 64 * HS;
@@ -351,14 +350,14 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
   const int h = cid.h, R = cid.R, C = cid.C;
-  const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
+  const int tid = threadIdx.x, slot = tid >> (L / 2), part = tid & (L - 1);
   const int w = geo.w, D = geo.D;
-  for (int i = tid; i < tabn; i += 128) tab[i] = table[(long long)i * geo.H + h];
+  for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
   if constexpr (TAB) {
     dst = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(smem) +
                                    ((reinterpret_cast<unsigned char*>(kfl + 64) - reinterpret_cast<unsigned char*>(smem) + 15) & ~15));
     acc = tpart + (long long)blockIdx.x * tabn;
-    for (int i = tid; i < tabn; i += 128) acc[i] = 0.f;
+    for (int i = tid; i < tabn; i += 64 * L) acc[i] = 0.f;
   }
 
   const int l = cid.piece * 64 + slot;
@@ -370,13 +369,13 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
   const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
   for (int it = 0; it < nimg; ++it) {
   const int b = cid.b + it * geo.nslice;
-  float qh[HH], doh[HH], dqh[HH];
+  float qh[HP], doh[HP], dqh[HP];
 #pragma unroll
-  for (int i = 0; i < HH; ++i) { qh[i] = 0.f; doh[i] = 0.f; dqh[i] = 0.f; }
+  for (int i = 0; i < HP; ++i) { qh[i] = 0.f; doh[i] = 0.f; dqh[i] = 0.f; }
   float lse_i = INFINITY, del_i = 0.f;
   if (qvalid) {
-    load_seg<T, HH>(row_ptr<T>(q, b, h, tokq), half * HH, D, qh);
-    load_seg<T, HH>(row_ptr<T>(d_o, b, h, tokq), half * HH, D, doh);
+    load_seg<T, HP>(row_ptr<T>(q, b, h, tokq), part * HP, D, qh);
+    load_seg<T, HP>(row_ptr<T>(d_o, b, h, tokq), part * HP, D, doh);
     lse_i = lse[((long long)b * geo.H + h) * geo.Nloc + tokq];
     del_i = delta[((long long)b * geo.H + h) * geo.Nloc + tokq];
   }
@@ -395,284 +394,13 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
       dR = geo.offR[oi]; dC = geo.offC[oi];
       KR = R + dR; KC = C + dC;
       if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
-      else if (KR < 0 || KR >= geo.mx || KC < 0 || KC >= geo.my) continue;
-    }
-    __syncthreads();
-    {
-      float kk[HH], vv[HH];
-#pragma unroll
-      for (int i = 0; i < HH; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
-      int flag = 0, vr = 0, vc = 0; long long tok = -1;
-      if (isg) {
-        const int t = pi * 64 + slot;
-        if (t < geo.g) { flag = 2; vr = t; tok = t; }
-      } else {
-        const int lk = kp * 64 + slot;
-        if (lk < geo.w2) {
-          const int kr = lk / w, kc = lk % w;
-          const int ar = KR * w + kr, ac = KC * w + kc;
-          const bool real = (ar < geo.nx) && (ac < geo.ny);
-          if (geo.exact == -1)
-            flag = !(((R + dR == geo.mx - 1) && (kr >= w - geo.padx)) ||
-                     ((C + dC == geo.my - 1) && (kc >= w - geo.pady)));
-          else
-            flag = real;
-          if (flag && real) tok = geo.g + (long long)ar * geo.ny + ac;
-          vr = dR * w + kr; vc = dC * w + kc;
-        }
-      }
-      if (tok >= 0) {
-        load_seg<T, HH>(row_ptr<T>(k, b, h, tok), half * HH, D, kk);
-        load_seg<T, HH>(row_ptr<T>(v, b, h, tok), half * HH, D, vv);
-      }
-      float* kd = Ks + slot * HS + TL::off(half);
-      float* vd = Vs + slot * HS + TL::off(half);
-#pragma unroll
-      for (int i = 0; i < HH; ++i) { kd[i] = kk[i]; vd[i] = vv[i]; }
-      if (half == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
-    }
-    __syncthreads();
-    for (int j = 0; j < 64; ++j) {
-      const int f = kfl[j];
-      if (!f) {
-        if (TAB && half == 0) dst[slot * kSimtDsLd + j] = 0.f;
-        continue;
-      }
-      float km = 1.f;                                    // dropout: keep / (1 - p) of the column
-      if constexpr (DROP) km = drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? geo.drop_scale : 0.f;
-      const float* kd = Ks + j * HS + TL::off(half);
-      const float* vd = Vs + j * HS + TL::off(half);
-      float sp = 0.f, dpp = 0.f;
-#pragma unroll
-      for (int i = 0; i < HH; ++i) { sp = fmaf(qh[i], kd[i], sp); dpp = fmaf(doh[i], vd[i], dpp); }
-      sp += __shfl_xor_sync(0xffffffffu, sp, 1);
-      dpp += __shfl_xor_sync(0xffffffffu, dpp, 1);
-      float bias = 0.f; bool ok = qvalid; int bidx = -1;
-      if (f == 2) {
-        if (geo.has_bias) bias = g2l[((long long)geo.H + h) * geo.g + kvr[j]];
-      } else {
-        const int dr = qr - kvr[j], dc = qc - kvc[j];
-        if (geo.exact == 1 && (abs(dr) > w || abs(dc) > w)) ok = false;
-        if (geo.has_bias && ok) { bidx = (dr + 2 * w - 1) * tw + dc + 2 * w - 1; bias = tab[bidx]; }
-      }
-      float tg = 0.f;                                    // TAB: this pair's term of the table gradient
-      if (ok) {
-        const float p = __expf(fmaf(geo.scale, sp, bias) - lse_i);
-        if constexpr (DROP) dpp *= km;
-        const float ds = p * (dpp - del_i);
-#pragma unroll
-        for (int i = 0; i < HH; ++i) dqh[i] = fmaf(ds, kd[i], dqh[i]);
-        if (bidx >= 0) tg = ds;
-      }
-      if (TAB && half == 0) dst[slot * kSimtDsLd + j] = tg;
-    }
-    if constexpr (TAB) {
-      if (!isg) {            // CTA-uniform; the next piece writes the tile only after its two barriers
-        __syncthreads();     // every query's dS is in the tile
-        table_grad_piece(dst, kSimtDsLd, acc, geo, dR, dC, cid.piece, kp);
-      }
-    }
-  }
-  if (qvalid) {
-#pragma unroll
-    for (int i = 0; i < HH; ++i) dqh[i] *= geo.scale;
-    store_seg<T, HH>(row_ptr_w<T>(dq, b, h, tokq), half * HH, D, dqh);
-  }
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// backward pass 2 (key-stationary): dk, dv of the LOCAL key rows.  CTA = one 64-key piece of one
-// key chunk; it walks the query chunks that visit it (the symmetric image of the offset list).
-// ----------------------------------------------------------------------------------------------
-template <typename T, int HD, bool DROP = false>
-__global__ void __launch_bounds__(128)
-simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
-             const float* __restrict__ delta, const float* __restrict__ table) {
-  using TL = Tile<HD>;
-  constexpr int HH = TL::HH, HS = TL::HS;
-  extern __shared__ float smem[];
-  float* Qs = smem;
-  float* Gs = Qs + 64 * HS;
-  float* tab = Gs + 64 * HS;
-  const int tw = 4 * geo.w - 1;
-  const int tabn = geo.has_bias ? tw * tw : 0;
-  float* lse_s = tab + tabn;
-  float* del_s = lse_s + 64;
-  short* qrs = reinterpret_cast<short*>(del_s + 64);
-  short* qcs = qrs + 64;
-  unsigned char* qfl = reinterpret_cast<unsigned char*>(qcs + 64);
-  int* qtok = reinterpret_cast<int*>(qfl + 64);            // DROP only: the query token of each staged column
-
-  const ChunkId cid = decode_block(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, KR = cid.R, KC = cid.C;
-  const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
-  const int w = geo.w, D = geo.D;
-  for (int i = tid; i < tabn; i += 128) tab[i] = table[(long long)i * geo.H + h];
-
-  const int lk = cid.piece * 64 + slot;
-  const int kr = lk / w, kc = lk % w;
-  const int ar = KR * w + kr, ac = KC * w + kc;
-  const bool kreal = (lk < geo.w2) && (ar < geo.nx) && (ac < geo.ny);
-  const long long tokk = geo.g + (long long)ar * geo.ny + ac;
-
-  float kh[HH], vh[HH], dkh[HH], dvh[HH];
-#pragma unroll
-  for (int i = 0; i < HH; ++i) { kh[i] = 0.f; vh[i] = 0.f; dkh[i] = 0.f; dvh[i] = 0.f; }
-  if (kreal) {
-    load_seg<T, HH>(row_ptr<T>(k, b, h, tokk), half * HH, D, kh);
-    load_seg<T, HH>(row_ptr<T>(v, b, h, tokk), half * HH, D, vh);
-  }
-
-  for (int oi = 0; oi < geo.noffs; ++oi) {
-    const int dR = geo.offR[oi], dC = geo.offC[oi];
-    int QR = KR - dR, QC = KC - dC;
-    if (geo.exact == -1) { QR = (QR + geo.mx) % geo.mx; QC = (QC + geo.my) % geo.my; }
-    else if (QR < 0 || QR >= geo.mx || QC < 0 || QC >= geo.my) continue;
-    // is this key visible from query chunk (QR,QC) through offset (dR,dC)?
-    bool kvis = kreal;
-    if (geo.exact == -1)
-      kvis = kreal && !(((QR + dR == geo.mx - 1) && (kr >= w - geo.padx)) ||
-                        ((QC + dC == geo.my - 1) && (kc >= w - geo.pady)));
-    const int vr = dR * w + kr, vc = dC * w + kc;
-    for (int qp = 0; qp < geo.npc; ++qp) {
-      __syncthreads();
-      {
-        float qq[HH], gg[HH];
-#pragma unroll
-        for (int i = 0; i < HH; ++i) { qq[i] = 0.f; gg[i] = 0.f; }
-        const int l = qp * 64 + slot;
-        const int qr = l / w, qc = l % w;
-        const int r = QR * w + qr, c = QC * w + qc;
-        const bool qv = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
-        if (qv) {
-          const long long tq = (long long)r * geo.ny + c;
-          load_seg<T, HH>(row_ptr<T>(q, b, h, tq), half * HH, D, qq);
-          load_seg<T, HH>(row_ptr<T>(d_o, b, h, tq), half * HH, D, gg);
-          if (half == 0) {
-            lse_s[slot] = lse[((long long)b * geo.H + h) * geo.Nloc + tq];
-            del_s[slot] = delta[((long long)b * geo.H + h) * geo.Nloc + tq];
-          }
-        }
-        float* qd = Qs + slot * HS + TL::off(half);
-        float* gd = Gs + slot * HS + TL::off(half);
-#pragma unroll
-        for (int i = 0; i < HH; ++i) { qd[i] = qq[i]; gd[i] = gg[i]; }
-        if (half == 0) { qrs[slot] = (short)qr; qcs[slot] = (short)qc; qfl[slot] = (unsigned char)qv; }
-        if (DROP && half == 0) qtok[slot] = r * geo.ny + c;
-      }
-      __syncthreads();
-      for (int i2 = 0; i2 < 64; ++i2) {
-        if (!qfl[i2]) continue;                              // warp-uniform
-        const float* qd = Qs + i2 * HS + TL::off(half);
-        const float* gd = Gs + i2 * HS + TL::off(half);
-        float sp = 0.f, dpp = 0.f;
-#pragma unroll
-        for (int i = 0; i < HH; ++i) { sp = fmaf(kh[i], qd[i], sp); dpp = fmaf(vh[i], gd[i], dpp); }
-        sp += __shfl_xor_sync(0xffffffffu, sp, 1);
-        dpp += __shfl_xor_sync(0xffffffffu, dpp, 1);
-        const int dr = qrs[i2] - vr, dc = qcs[i2] - vc;
-        bool ok = kvis;
-        if (geo.exact == 1 && (abs(dr) > w || abs(dc) > w)) ok = false;
-        if (ok) {
-          const float bias = geo.has_bias ? tab[(dr + 2 * w - 1) * tw + dc + 2 * w - 1] : 0.f;
-          float p = __expf(fmaf(geo.scale, sp, bias) - lse_s[i2]);
-          if constexpr (DROP) {            // dS = P (dP keep / (1 - p) - delta), dV += P keep / (1 - p) dO
-            const float km = drop_keep(geo, (uint32_t)qtok[i2], (uint32_t)(geo.g + oi * geo.w2 + lk), 2u * (uint32_t)(b * geo.H + h))
-                                 ? geo.drop_scale : 0.f;
-            const float ds = p * (dpp * km - del_s[i2]);
-            p *= km;
-#pragma unroll
-            for (int i = 0; i < HH; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
-          } else {
-            const float ds = p * (dpp - del_s[i2]);
-#pragma unroll
-            for (int i = 0; i < HH; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
-          }
-        }
-      }
-    }
-  }
-  if (kreal) {
-#pragma unroll
-    for (int i = 0; i < HH; ++i) dkh[i] *= geo.scale;
-    store_seg<T, HH>(row_ptr_w<T>(dk, b, h, tokk), half * HH, D, dkh);
-    store_seg<T, HH>(row_ptr_w<T>(dv, b, h, tokk), half * HH, D, dvh);
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// Four lanes per row: the fp32 training kernels at 64 < D <= 128 (HD 128).  With a thread pair per row every thread
-// would hold HD/2 = 64 floats per row tensor (192 in pass 1, 256 in pass 2) and spill.  Here lane `qt` = tid & 3 of a
-// slot owns the 32 consecutive channels [32 qt, 32 qt + 32) of its row, a dot product is its 32-term FMA chain plus two
-// shuffle steps (group_sum<4>), and a 256-thread CTA covers the same 64-slot piece as the two-lane kernels: the grids,
-// the workspace and the fixed order of the table gradient are theirs.  Per-row values (lse, delta, the dS tile, the
-// staged key / query metadata) are written by lane 0 of each slot.
-// ----------------------------------------------------------------------------------------------
-// fp32 smem tile row: four quarters of HD/4 floats at a stride of HD/4 + 1, so the four lanes of a row hit four banks,
-// and the 8 rows a warp stages hit all 32 (the row stride HD + 4 is 4 banks).
-template <int HD> struct Tile4 {
-  static constexpr int HQ = HD / 4;
-  static constexpr int HS = HD + 4;
-  static __device__ __forceinline__ int off(int qt) { return qt * (HQ + 1); }
-};
-
-// forward, local queries (instantiated for dropout: the two-lane kernel serves the forward without it)
-template <typename T, int HD, bool DROP>
-__global__ void __launch_bounds__(256, 1)
-simt_fwd_local4(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
-                const float* __restrict__ table, const float* __restrict__ g2l) {
-  using TL = Tile4<HD>;
-  constexpr int HQ = TL::HQ, HS = TL::HS;
-  extern __shared__ float smem[];
-  float* Ks = smem;
-  float* Vs = Ks + 64 * HS;
-  float* tab = Vs + 64 * HS;
-  const int tw = 4 * geo.w - 1;
-  const int tabn = geo.has_bias ? tw * tw : 0;
-  short* kvr = reinterpret_cast<short*>(tab + tabn);
-  short* kvc = kvr + 64;
-  unsigned char* kfl = reinterpret_cast<unsigned char*>(kvc + 64);
-
-  const ChunkId cid = decode_block(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
-  const int tid = threadIdx.x, slot = tid >> 2, qt = tid & 3;
-  const int w = geo.w, D = geo.D;
-
-  for (int i = tid; i < tabn; i += 256) tab[i] = table[(long long)i * geo.H + h];
-
-  const int l = cid.piece * 64 + slot;
-  const int qr = l / w, qc = l % w;
-  const int r = R * w + qr, c = C * w + qc;
-  const bool qvalid = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
-
-  float qh[HQ], oh[HQ];
-#pragma unroll
-  for (int i = 0; i < HQ; ++i) { qh[i] = 0.f; oh[i] = 0.f; }
-  if (qvalid) load_seg<T, HQ>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), qt * HQ, D, qh);
-  float m = -INFINITY, lsum = 0.f;
-  const uint32_t drow = (uint32_t)(r * geo.ny + c), dsid = 2u * (uint32_t)(b * geo.H + h);   // dropout: row, stream 0
-
-  const int ngp = (geo.g + 63) / 64;
-  const int npieces = ngp + geo.noffs * geo.npc;
-  for (int pi = 0; pi < npieces; ++pi) {
-    const bool isg = pi < ngp;
-    int dR = 0, dC = 0, KR = 0, KC = 0, kp = 0;
-    int cbase = pi * 64;                  // dropout: attn1 column of the piece's slot 0
-    if (!isg) {
-      const int oi = (pi - ngp) / geo.npc;
-      kp = (pi - ngp) % geo.npc;
-      if (DROP) cbase = geo.g + oi * geo.w2 + kp * 64;
-      dR = geo.offR[oi]; dC = geo.offC[oi];
-      KR = R + dR; KC = C + dC;
-      if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
       else if (KR < 0 || KR >= geo.mx || KC < 0 || KC >= geo.my) continue;   // CTA-uniform
     }
     __syncthreads();
-    {   // stage one piece of <=64 keys: lane qt of a slot loads a quarter row of K and V
-      float kk[HQ], vv[HQ];
+    {
+      float kk[HP], vv[HP];
 #pragma unroll
-      for (int i = 0; i < HQ; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
+      for (int i = 0; i < HP; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
       int flag = 0, vr = 0, vc = 0; long long tok = -1;
       if (isg) {
         const int t = pi * 64 + slot;
@@ -693,180 +421,33 @@ simt_fwd_local4(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
         }
       }
       if (tok >= 0) {
-        load_seg<T, HQ>(row_ptr<T>(k, b, h, tok), qt * HQ, D, kk);
-        load_seg<T, HQ>(row_ptr<T>(v, b, h, tok), qt * HQ, D, vv);
+        load_seg<T, HP>(row_ptr<T>(k, b, h, tok), part * HP, D, kk);
+        load_seg<T, HP>(row_ptr<T>(v, b, h, tok), part * HP, D, vv);
       }
-      float* kd = Ks + slot * HS + TL::off(qt);
-      float* vd = Vs + slot * HS + TL::off(qt);
+      float* kd = Ks + slot * HS + TL::off(part);
+      float* vd = Vs + slot * HS + TL::off(part);
 #pragma unroll
-      for (int i = 0; i < HQ; ++i) { kd[i] = kk[i]; vd[i] = vv[i]; }
-      if (qt == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
-    }
-    __syncthreads();
-    for (int j = 0; j < 64; ++j) {
-      const int f = kfl[j];
-      if (!f) continue;                                   // warp-uniform
-      const float* kd = Ks + j * HS + TL::off(qt);
-      float sp = 0.f;
-#pragma unroll
-      for (int i = 0; i < HQ; ++i) sp = fmaf(qh[i], kd[i], sp);
-      sp = group_sum<4>(sp);
-      float bias = 0.f; bool ok = qvalid;
-      if (f == 2) {
-        if (geo.has_bias) bias = g2l[((long long)geo.H + h) * geo.g + kvr[j]];
-      } else {
-        const int dr = qr - kvr[j], dc = qc - kvc[j];
-        if (geo.exact == 1 && (abs(dr) > w || abs(dc) > w)) ok = false;
-        if (geo.has_bias && ok) bias = tab[(dr + 2 * w - 1) * tw + dc + 2 * w - 1];
-      }
-      if (ok) {
-        const float s = fmaf(geo.scale, sp, bias);
-        const float* vd = Vs + j * HS + TL::off(qt);
-        // dropout: lsum sums the undropped P; O sums P * keep, scaled by 1 / (1 - p) at the end
-        const float km = DROP ? (drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? 1.f : 0.f) : 1.f;
-        if (s > m) {
-          const float corr = __expf(m - s);
-          lsum = lsum * corr + 1.f;
-#pragma unroll
-          for (int i = 0; i < HQ; ++i) oh[i] = fmaf(oh[i], corr, km * vd[i]);
-          m = s;
-        } else {
-          const float p = __expf(s - m);
-          lsum += p;
-#pragma unroll
-          for (int i = 0; i < HQ; ++i) oh[i] = fmaf(p * km, vd[i], oh[i]);
-        }
-      }
-    }
-  }
-  if (qvalid) {
-    const float inv = (lsum > 0.f ? 1.f / lsum : 0.f) * (DROP ? geo.drop_scale : 1.f);
-#pragma unroll
-    for (int i = 0; i < HQ; ++i) oh[i] *= inv;
-    const long long tokq = (long long)r * geo.ny + c;
-    store_seg<T, HQ>(row_ptr_w<T>(o, b, h, tokq), qt * HQ, D, oh);
-    if (qt == 0) lse[((long long)b * geo.H + h) * geo.Nloc + tokq] = m + logf(lsum);
-  }
-}
-
-// backward pass 1 (query-stationary): dq and, with the table (TAB), its partials; simt_bwd_dq with four lanes per row
-template <typename T, int HD, bool DROP = false, bool TAB = false>
-__global__ void __launch_bounds__(256, 1)
-simt_bwd_dq4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse,
-             const float* __restrict__ delta, const float* __restrict__ table,
-             const float* __restrict__ g2l, float* __restrict__ tpart) {
-  using TL = Tile4<HD>;
-  constexpr int HQ = TL::HQ, HS = TL::HS;
-  extern __shared__ float smem[];
-  float* Ks = smem;
-  float* Vs = Ks + 64 * HS;
-  float* tab = Vs + 64 * HS;
-  const int tw = 4 * geo.w - 1;
-  const int tabn = geo.has_bias ? tw * tw : 0;
-  short* kvr = reinterpret_cast<short*>(tab + tabn);
-  short* kvc = kvr + 64;
-  unsigned char* kfl = reinterpret_cast<unsigned char*>(kvc + 64);
-  float* dst = nullptr;                                   // TAB: the dS tile, 16-byte aligned after kfl
-  float* acc = nullptr;                                   // TAB: the CTA's row of table partials
-
-  const ChunkId cid = decode_block(geo, blockIdx.x);
-  const int h = cid.h, R = cid.R, C = cid.C;
-  const int tid = threadIdx.x, slot = tid >> 2, qt = tid & 3;
-  const int w = geo.w, D = geo.D;
-  for (int i = tid; i < tabn; i += 256) tab[i] = table[(long long)i * geo.H + h];
-  if constexpr (TAB) {
-    dst = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(smem) +
-                                   ((reinterpret_cast<unsigned char*>(kfl + 64) - reinterpret_cast<unsigned char*>(smem) + 15) & ~15));
-    acc = tpart + (long long)blockIdx.x * tabn;
-    for (int i = tid; i < tabn; i += 256) acc[i] = 0.f;
-  }
-
-  const int l = cid.piece * 64 + slot;
-  const int qr = l / w, qc = l % w;
-  const int r = R * w + qr, c = C * w + qc;
-  const bool qvalid = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
-  const long long tokq = (long long)r * geo.ny + c;
-
-  const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
-  for (int it = 0; it < nimg; ++it) {
-  const int b = cid.b + it * geo.nslice;
-  float qh[HQ], doh[HQ], dqh[HQ];
-#pragma unroll
-  for (int i = 0; i < HQ; ++i) { qh[i] = 0.f; doh[i] = 0.f; dqh[i] = 0.f; }
-  float lse_i = INFINITY, del_i = 0.f;
-  if (qvalid) {
-    load_seg<T, HQ>(row_ptr<T>(q, b, h, tokq), qt * HQ, D, qh);
-    load_seg<T, HQ>(row_ptr<T>(d_o, b, h, tokq), qt * HQ, D, doh);
-    lse_i = lse[((long long)b * geo.H + h) * geo.Nloc + tokq];
-    del_i = delta[((long long)b * geo.H + h) * geo.Nloc + tokq];
-  }
-  const uint32_t drow = (uint32_t)tokq, dsid = 2u * (uint32_t)(b * geo.H + h);   // dropout: row, stream 0
-
-  const int ngp = (geo.g + 63) / 64;
-  const int npieces = ngp + geo.noffs * geo.npc;
-  for (int pi = 0; pi < npieces; ++pi) {
-    const bool isg = pi < ngp;
-    int dR = 0, dC = 0, KR = 0, KC = 0, kp = 0;
-    int cbase = pi * 64;                  // dropout: attn1 column of the piece's slot 0
-    if (!isg) {
-      const int oi = (pi - ngp) / geo.npc;
-      kp = (pi - ngp) % geo.npc;
-      if (DROP) cbase = geo.g + oi * geo.w2 + kp * 64;
-      dR = geo.offR[oi]; dC = geo.offC[oi];
-      KR = R + dR; KC = C + dC;
-      if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
-      else if (KR < 0 || KR >= geo.mx || KC < 0 || KC >= geo.my) continue;
-    }
-    __syncthreads();
-    {
-      float kk[HQ], vv[HQ];
-#pragma unroll
-      for (int i = 0; i < HQ; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
-      int flag = 0, vr = 0, vc = 0; long long tok = -1;
-      if (isg) {
-        const int t = pi * 64 + slot;
-        if (t < geo.g) { flag = 2; vr = t; tok = t; }
-      } else {
-        const int lk = kp * 64 + slot;
-        if (lk < geo.w2) {
-          const int kr = lk / w, kc = lk % w;
-          const int ar = KR * w + kr, ac = KC * w + kc;
-          const bool real = (ar < geo.nx) && (ac < geo.ny);
-          if (geo.exact == -1)
-            flag = !(((R + dR == geo.mx - 1) && (kr >= w - geo.padx)) ||
-                     ((C + dC == geo.my - 1) && (kc >= w - geo.pady)));
-          else
-            flag = real;
-          if (flag && real) tok = geo.g + (long long)ar * geo.ny + ac;
-          vr = dR * w + kr; vc = dC * w + kc;
-        }
-      }
-      if (tok >= 0) {
-        load_seg<T, HQ>(row_ptr<T>(k, b, h, tok), qt * HQ, D, kk);
-        load_seg<T, HQ>(row_ptr<T>(v, b, h, tok), qt * HQ, D, vv);
-      }
-      float* kd = Ks + slot * HS + TL::off(qt);
-      float* vd = Vs + slot * HS + TL::off(qt);
-#pragma unroll
-      for (int i = 0; i < HQ; ++i) { kd[i] = kk[i]; vd[i] = vv[i]; }
-      if (qt == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
+      for (int i = 0; i < HP; ++i) { kd[i] = kk[i]; vd[i] = vv[i]; }
+      if (part == 0) { kvr[slot] = (short)vr; kvc[slot] = (short)vc; kfl[slot] = (unsigned char)flag; }
     }
     __syncthreads();
     for (int j = 0; j < 64; ++j) {
       const int f = kfl[j];
       if (!f) {
-        if (TAB && qt == 0) dst[slot * kSimtDsLd + j] = 0.f;
+        if (TAB && part == 0) dst[slot * kSimtDsLd + j] = 0.f;
         continue;
       }
       float km = 1.f;                                    // dropout: keep / (1 - p) of the column
       if constexpr (DROP) km = drop_keep(geo, drow, (uint32_t)(cbase + j), dsid) ? geo.drop_scale : 0.f;
-      const float* kd = Ks + j * HS + TL::off(qt);
-      const float* vd = Vs + j * HS + TL::off(qt);
+      const float* kd = Ks + j * HS + TL::off(part);
+      const float* vd = Vs + j * HS + TL::off(part);
       float sp = 0.f, dpp = 0.f;
 #pragma unroll
-      for (int i = 0; i < HQ; ++i) { sp = fmaf(qh[i], kd[i], sp); dpp = fmaf(doh[i], vd[i], dpp); }
-      sp = group_sum<4>(sp);
-      dpp = group_sum<4>(dpp);
+      for (int i = 0; i < HP; ++i) { sp = fmaf(qh[i], kd[i], sp); dpp = fmaf(doh[i], vd[i], dpp); }
+      sp += __shfl_xor_sync(0xffffffffu, sp, 1);           // over the L lanes of the row
+      if constexpr (L == 4) sp += __shfl_xor_sync(0xffffffffu, sp, 2);
+      dpp += __shfl_xor_sync(0xffffffffu, dpp, 1);
+      if constexpr (L == 4) dpp += __shfl_xor_sync(0xffffffffu, dpp, 2);
       float bias = 0.f; bool ok = qvalid; int bidx = -1;
       if (f == 2) {
         if (geo.has_bias) bias = g2l[((long long)geo.H + h) * geo.g + kvr[j]];
@@ -881,33 +462,36 @@ simt_bwd_dq4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__
         if constexpr (DROP) dpp *= km;
         const float ds = p * (dpp - del_i);
 #pragma unroll
-        for (int i = 0; i < HQ; ++i) dqh[i] = fmaf(ds, kd[i], dqh[i]);
+        for (int i = 0; i < HP; ++i) dqh[i] = fmaf(ds, kd[i], dqh[i]);
         if (bidx >= 0) tg = ds;
       }
-      if (TAB && qt == 0) dst[slot * kSimtDsLd + j] = tg;
+      if (TAB && part == 0) dst[slot * kSimtDsLd + j] = tg;
     }
     if constexpr (TAB) {
       if (!isg) {            // CTA-uniform; the next piece writes the tile only after its two barriers
         __syncthreads();     // every query's dS is in the tile
-        table_grad_piece(dst, kSimtDsLd, acc, geo, dR, dC, cid.piece, kp, 256);
+        table_grad_piece(dst, kSimtDsLd, acc, geo, dR, dC, cid.piece, kp, 64 * L);
       }
     }
   }
   if (qvalid) {
 #pragma unroll
-    for (int i = 0; i < HQ; ++i) dqh[i] *= geo.scale;
-    store_seg<T, HQ>(row_ptr_w<T>(dq, b, h, tokq), qt * HQ, D, dqh);
+    for (int i = 0; i < HP; ++i) dqh[i] *= geo.scale;
+    store_seg<T, HP>(row_ptr_w<T>(dq, b, h, tokq), part * HP, D, dqh);
   }
   }
 }
 
-// backward pass 2 (key-stationary): dk, dv of the local key rows; simt_bwd_dkv with four lanes per row
-template <typename T, int HD, bool DROP = false>
-__global__ void __launch_bounds__(256, 1)
-simt_bwd_dkv4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
-              const float* __restrict__ delta, const float* __restrict__ table) {
-  using TL = Tile4<HD>;
-  constexpr int HQ = TL::HQ, HS = TL::HS;
+// ----------------------------------------------------------------------------------------------
+// backward pass 2 (key-stationary): dk, dv of the LOCAL key rows.  CTA = one 64-key piece of one
+// key chunk; it walks the query chunks that visit it (the symmetric image of the offset list).
+// ----------------------------------------------------------------------------------------------
+template <typename T, int HD, int L, bool DROP>
+__global__ void __launch_bounds__(64 * L, L == 4 ? 1 : 0)
+simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
+             const float* __restrict__ delta, const float* __restrict__ table) {
+  using TL = Tile<HD, L>;
+  constexpr int HP = TL::HP, HS = TL::HS;
   extern __shared__ float smem[];
   float* Qs = smem;
   float* Gs = Qs + 64 * HS;
@@ -923,9 +507,9 @@ simt_bwd_dkv4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
   const int b = cid.b, h = cid.h, KR = cid.R, KC = cid.C;
-  const int tid = threadIdx.x, slot = tid >> 2, qt = tid & 3;
+  const int tid = threadIdx.x, slot = tid >> (L / 2), part = tid & (L - 1);
   const int w = geo.w, D = geo.D;
-  for (int i = tid; i < tabn; i += 256) tab[i] = table[(long long)i * geo.H + h];
+  for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
 
   const int lk = cid.piece * 64 + slot;
   const int kr = lk / w, kc = lk % w;
@@ -933,12 +517,12 @@ simt_bwd_dkv4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
   const bool kreal = (lk < geo.w2) && (ar < geo.nx) && (ac < geo.ny);
   const long long tokk = geo.g + (long long)ar * geo.ny + ac;
 
-  float kh[HQ], vh[HQ], dkh[HQ], dvh[HQ];
+  float kh[HP], vh[HP], dkh[HP], dvh[HP];
 #pragma unroll
-  for (int i = 0; i < HQ; ++i) { kh[i] = 0.f; vh[i] = 0.f; dkh[i] = 0.f; dvh[i] = 0.f; }
+  for (int i = 0; i < HP; ++i) { kh[i] = 0.f; vh[i] = 0.f; dkh[i] = 0.f; dvh[i] = 0.f; }
   if (kreal) {
-    load_seg<T, HQ>(row_ptr<T>(k, b, h, tokk), qt * HQ, D, kh);
-    load_seg<T, HQ>(row_ptr<T>(v, b, h, tokk), qt * HQ, D, vh);
+    load_seg<T, HP>(row_ptr<T>(k, b, h, tokk), part * HP, D, kh);
+    load_seg<T, HP>(row_ptr<T>(v, b, h, tokk), part * HP, D, vh);
   }
 
   for (int oi = 0; oi < geo.noffs; ++oi) {
@@ -955,39 +539,41 @@ simt_bwd_dkv4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
     for (int qp = 0; qp < geo.npc; ++qp) {
       __syncthreads();
       {
-        float qq[HQ], gg[HQ];
+        float qq[HP], gg[HP];
 #pragma unroll
-        for (int i = 0; i < HQ; ++i) { qq[i] = 0.f; gg[i] = 0.f; }
+        for (int i = 0; i < HP; ++i) { qq[i] = 0.f; gg[i] = 0.f; }
         const int l = qp * 64 + slot;
         const int qr = l / w, qc = l % w;
         const int r = QR * w + qr, c = QC * w + qc;
         const bool qv = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
         if (qv) {
           const long long tq = (long long)r * geo.ny + c;
-          load_seg<T, HQ>(row_ptr<T>(q, b, h, tq), qt * HQ, D, qq);
-          load_seg<T, HQ>(row_ptr<T>(d_o, b, h, tq), qt * HQ, D, gg);
-          if (qt == 0) {
+          load_seg<T, HP>(row_ptr<T>(q, b, h, tq), part * HP, D, qq);
+          load_seg<T, HP>(row_ptr<T>(d_o, b, h, tq), part * HP, D, gg);
+          if (part == 0) {
             lse_s[slot] = lse[((long long)b * geo.H + h) * geo.Nloc + tq];
             del_s[slot] = delta[((long long)b * geo.H + h) * geo.Nloc + tq];
           }
         }
-        float* qd = Qs + slot * HS + TL::off(qt);
-        float* gd = Gs + slot * HS + TL::off(qt);
+        float* qd = Qs + slot * HS + TL::off(part);
+        float* gd = Gs + slot * HS + TL::off(part);
 #pragma unroll
-        for (int i = 0; i < HQ; ++i) { qd[i] = qq[i]; gd[i] = gg[i]; }
-        if (qt == 0) { qrs[slot] = (short)qr; qcs[slot] = (short)qc; qfl[slot] = (unsigned char)qv; }
-        if (DROP && qt == 0) qtok[slot] = r * geo.ny + c;
+        for (int i = 0; i < HP; ++i) { qd[i] = qq[i]; gd[i] = gg[i]; }
+        if (part == 0) { qrs[slot] = (short)qr; qcs[slot] = (short)qc; qfl[slot] = (unsigned char)qv; }
+        if (DROP && part == 0) qtok[slot] = r * geo.ny + c;
       }
       __syncthreads();
       for (int i2 = 0; i2 < 64; ++i2) {
         if (!qfl[i2]) continue;                              // warp-uniform
-        const float* qd = Qs + i2 * HS + TL::off(qt);
-        const float* gd = Gs + i2 * HS + TL::off(qt);
+        const float* qd = Qs + i2 * HS + TL::off(part);
+        const float* gd = Gs + i2 * HS + TL::off(part);
         float sp = 0.f, dpp = 0.f;
 #pragma unroll
-        for (int i = 0; i < HQ; ++i) { sp = fmaf(kh[i], qd[i], sp); dpp = fmaf(vh[i], gd[i], dpp); }
-        sp = group_sum<4>(sp);
-        dpp = group_sum<4>(dpp);
+        for (int i = 0; i < HP; ++i) { sp = fmaf(kh[i], qd[i], sp); dpp = fmaf(vh[i], gd[i], dpp); }
+        sp += __shfl_xor_sync(0xffffffffu, sp, 1);           // over the L lanes of the row
+        if constexpr (L == 4) sp += __shfl_xor_sync(0xffffffffu, sp, 2);
+        dpp += __shfl_xor_sync(0xffffffffu, dpp, 1);
+        if constexpr (L == 4) dpp += __shfl_xor_sync(0xffffffffu, dpp, 2);
         const int dr = qrs[i2] - vr, dc = qcs[i2] - vc;
         bool ok = kvis;
         if (geo.exact == 1 && (abs(dr) > w || abs(dc) > w)) ok = false;
@@ -1000,11 +586,11 @@ simt_bwd_dkv4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
             const float ds = p * (dpp * km - del_s[i2]);
             p *= km;
 #pragma unroll
-            for (int i = 0; i < HQ; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
+            for (int i = 0; i < HP; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
           } else {
             const float ds = p * (dpp - del_s[i2]);
 #pragma unroll
-            for (int i = 0; i < HQ; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
+            for (int i = 0; i < HP; ++i) { dkh[i] = fmaf(ds, qd[i], dkh[i]); dvh[i] = fmaf(p, gd[i], dvh[i]); }
           }
         }
       }
@@ -1012,9 +598,9 @@ simt_bwd_dkv4(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
   }
   if (kreal) {
 #pragma unroll
-    for (int i = 0; i < HQ; ++i) dkh[i] *= geo.scale;
-    store_seg<T, HQ>(row_ptr_w<T>(dk, b, h, tokk), qt * HQ, D, dkh);
-    store_seg<T, HQ>(row_ptr_w<T>(dv, b, h, tokk), qt * HQ, D, dvh);
+    for (int i = 0; i < HP; ++i) dkh[i] *= geo.scale;
+    store_seg<T, HP>(row_ptr_w<T>(dk, b, h, tokk), part * HP, D, dkh);
+    store_seg<T, HP>(row_ptr_w<T>(dv, b, h, tokk), part * HP, D, dvh);
   }
 }
 

@@ -589,7 +589,7 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
       if (pi >= ngp) {       // a chunk piece (CTA-uniform); the tile is rewritten only after the next round's barrier
         __syncthreads();     // every thread's dS is in the tile
         const int c = pi - ngp, vi = c / geo.npc;
-        table_grad_piece(dst, kDsLd, acc, geo, vl[vi].dR, vl[vi].dC, cid.piece, c - vi * geo.npc);
+        table_grad_piece(dst, kDsLd, acc, geo, vl[vi].dR, vl[vi].dC, cid.piece, c - vi * geo.npc, kThreads);
       }
     }
   }
