@@ -54,11 +54,13 @@ enum { VIL_F32 = 0, VIL_BF16 = 1, VIL_F16 = 2 };
 
 /* kernel family selection */
 enum {
-  VIL_IMPL_AUTO    = 0, /* wgmma path when the configuration is covered, else SIMT */
+  VIL_IMPL_AUTO    = 0, /* wgmma path when the configuration is covered, else SIMT; fp32 takes the wgmma path only
+                           with VIL_FLAG_F32_SPLIT */
   VIL_IMPL_SIMT    = 1, /* CUDA-core fp32 path: every (w, exact, mode, nglo) incl. fp32 I/O; forward D <= 128;
-                           backward and dropout D <= 128 in fp32, D <= 64 in bf16 / fp16 */
+                           backward and dropout D <= 128 in fp32, D <= 64 in bf16 / fp16.  Ignores VIL_FLAG_F32_SPLIT */
   VIL_IMPL_WGMMA   = 2  /* wgmma tensor-core path (bf16/fp16, D <= 128 with D % 8 == 0 and 16-byte-aligned rows; with
-                           the bias table w <= 42 when D > 64): error if the configuration is not covered */
+                           the bias table w <= 42 when D > 64; fp32 with VIL_FLAG_F32_SPLIT, below): error if the
+                           configuration is not covered */
 };
 
 /* VilAttnParams.flags */
@@ -69,7 +71,16 @@ enum {
      wgmma family only. */
   VIL_FLAG_F32_OUT = 1,
   /* accepted for ABI compatibility: every family runs one pipeline, so it changes nothing */
-  VIL_FLAG_UNFUSED = 2
+  VIL_FLAG_UNFUSED = 2,
+  /* fp32 operands may run on the wgmma tensor cores as split bf16 products (torch's
+     set_float32_matmul_precision("high") / ("medium")): each fp32 x is hi = bf16(x) plus lo = bf16(x - hi), and each
+     product A B is A_hi B_hi + A_hi B_lo + A_lo B_hi in fp32 accumulators (about 16 significant bits per term, against
+     the SIMT family's full fp32).  dtype must be VIL_F32 (else VIL_E_BADARG).  Covered: D <= 64 with D % 8 == 0 and
+     16-byte-aligned fp32 rows; with the bias table w <= 42 when D > 32.  VIL_IMPL_AUTO runs the split wgmma kernels where
+     they cover the call and the SIMT family elsewhere; VIL_IMPL_WGMMA fails where they do not; VIL_IMPL_SIMT ignores the
+     flag.  The backward must be given the flag of its forward.  The bit leaves VilAttnParams as it was, so the ABI version
+     stays 3: a library that predates the flag refuses it as an unknown bit (VIL_E_BADARG) rather than misreading it. */
+  VIL_FLAG_F32_SPLIT = 4
 };
 
 /* error codes */
@@ -160,13 +171,15 @@ int64_t     vil_attn_launch_count(void);
 /* name of the kernel family the last successful fwd / bwd call on this thread used ("simt" / "wgmma") */
 const char* vil_attn_last_impl(void);
 /* name of the main kernel the last wgmma forward / backward launch on this thread used ("wgmma_fwd", "wgmma_bwd";
-   "" when the family does not report one) - lets tests assert which variant ran */
+   "wgmma_f32split_fwd", "wgmma_f32split_bwd" for the split fp32 kernels; "" when the family does not report one) - lets
+   tests assert which variant ran */
 const char* vil_attn_last_kernel(void);
 
 /* scratch size needed by the forward (backward == 0) or backward (backward != 0) call; < 0 on error */
 int64_t vil_attn_workspace_bytes(const VilAttnParams* p, int backward);
 
-/* returns 1 if the wgmma family covers this configuration, 0 if only the SIMT family does, < 0 on error */
+/* returns 1 if the wgmma family covers this configuration (the split fp32 kernels when flags has VIL_FLAG_F32_SPLIT),
+   0 if only the SIMT family does, < 0 on error */
 int vil_attn_wgmma_supported(const VilAttnParams* p);
 
 /* fused forward: o, og, lse, lse_g.  `stream` is a cudaStream_t. */

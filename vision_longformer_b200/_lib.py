@@ -18,7 +18,7 @@ VIL_F32, VIL_BF16, VIL_F16 = 0, 1, 2
 VIL_IMPL_AUTO, VIL_IMPL_SIMT, VIL_IMPL_WGMMA = 0, 1, 2
 VIL_E_BADARG, VIL_E_UNSUPPORTED, VIL_E_CUDA, VIL_E_WORKSPACE = -1, -2, -3, -4
 ABI_VERSION = 3
-VIL_FLAG_F32_OUT, VIL_FLAG_UNFUSED = 1, 2
+VIL_FLAG_F32_OUT, VIL_FLAG_UNFUSED, VIL_FLAG_F32_SPLIT = 1, 2, 4
 
 # every symbol include/vil_attn.h declares
 EXPORTS = (

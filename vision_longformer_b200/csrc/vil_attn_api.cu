@@ -50,9 +50,11 @@ int make_geo(const VilAttnParams* p, vil::Geo* g) {
   if (p->exact != 0 && p->exact != 1 && p->exact != -1)
     return fail(VIL_E_BADARG, "longsc exact should be in [0,1,-1]!");
   if (p->mode < -1 || p->mode > 8) return fail(VIL_E_BADARG, "mode must be in [-1, 8]");
-  if (p->flags & ~(VIL_FLAG_F32_OUT | VIL_FLAG_UNFUSED)) return fail(VIL_E_BADARG, "unknown bits in flags");
+  if (p->flags & ~(VIL_FLAG_F32_OUT | VIL_FLAG_UNFUSED | VIL_FLAG_F32_SPLIT)) return fail(VIL_E_BADARG, "unknown bits in flags");
   if ((p->flags & VIL_FLAG_F32_OUT) && p->dtype == VIL_F32)
     return fail(VIL_E_BADARG, "VIL_FLAG_F32_OUT is the parity build of the bf16 / fp16 kernels; dtype is already fp32");
+  if ((p->flags & VIL_FLAG_F32_SPLIT) && p->dtype != VIL_F32)
+    return fail(VIL_E_BADARG, "VIL_FLAG_F32_SPLIT applies to fp32 operands only (dtype must be VIL_F32)");
   // the exact mask has 9*w^2 columns only: exact=1 with mode != 0 raises in the reference (:331-343)
   if (p->exact == 1 && p->mode != 0)
     return fail(VIL_E_BADARG, "exact sliding window (exact=1) only supports mode=0");

@@ -24,6 +24,7 @@ inline T4 t4(const VilTensor4& t) { T4 r; r.p = static_cast<char*>(t.ptr); r.sb 
 
 // flags of VilAttnParams
 inline bool out_f32(const VilAttnParams* p) { return (p->flags & VIL_FLAG_F32_OUT) != 0; }
+inline bool split_f32(const VilAttnParams* p) { return (p->flags & VIL_FLAG_F32_SPLIT) != 0; }
 
 // the backward workspace at float offset `off` (vil_common.cuh: ws_off_*)
 inline float* ws_at(const VilAttnParams* p, long long off) { return static_cast<float*>(p->workspace) + off; }

@@ -1,4 +1,5 @@
-// Tensor-core (wgmma) kernel family of the Vision-Longformer attention, bf16 / fp16 operands, fp32 accumulation.
+// Tensor-core (wgmma) kernel family of the Vision-Longformer attention, bf16 / fp16 operands, fp32 accumulation; fp32
+// operands run as split bf16 pairs (T = float, below).
 //
 // Same decomposition and masking rules as the SIMT family (vil_simt.cuh), with every product on the tensor cores:
 // a CTA is one warpgroup (128 threads) owning a 64-row tile; it walks 64-column pieces (the global keys, then the
@@ -44,10 +45,22 @@ __device__ __forceinline__ int acc_col(int i) { return ((i >> 2) << 3) + ((threa
 // two 16 KB tiles and 2 stages keep two CTAs on an SM (3 would leave one, DESIGN.md section 3).
 template <int HD> constexpr int kStages = HD <= 64 ? 3 : 2;
 
+// fp32 operands as split bf16 pairs (VIL_FLAG_F32_SPLIT): with T = float every product A B runs as
+// A_hi B_hi + A_hi B_lo + A_lo B_hi, hi = bf16(x), lo = bf16(x - hi), all three into the same fp32 accumulators.  A
+// (64 x HD) fp32 tile holds the hi tile in its first half and the lo tile in its second, each in the core-matrix layout
+// of a bf16 tile.  Such a tile has the bytes of a bf16 tile of head width 2 HD (kTileHD), and takes that tile's ring
+// depth and CTAs per SM.
+template <typename T> constexpr bool kSplit = std::is_same<T, float>::value;
+template <typename T> using Op = std::conditional_t<kSplit<T>, __nv_bfloat16, T>;   // element type of the products
+template <typename T, int HD> constexpr int kTileHD = kSplit<T> ? 2 * HD : HD;
+template <typename T, int HD> constexpr int kRing = kStages<kTileHD<T, HD>>;
+
 // The thread's row segment of a (64 x HD) tile: row `row`, columns [half HD / 2, (half + 1) HD / 2), copied 16 bytes at a
 // time from row `tok` of the (b, h) slice `base` (row stride st) straight into the core-matrix layout.  tok < 0 (a phantom
 // row) and 8-column groups at or past D are zero-filled without a read: padding keys / queries keep K = V = 0, which the
 // masks rely on (a NaN in a masked column would survive the fmaf with -inf).  Needs D % 8 == 0 and 16-byte aligned rows.
+// A split fp32 tile takes the 8 values of a core-matrix row as two 16-byte copies: the first four into the bytes of
+// their hi row, the last four into those of their lo row, where split_row converts them in place.
 template <typename T, int HD>
 __device__ __forceinline__ void stage_row(T* tile, const T* base, long long st, long long tok, int row, int half, int D) {
   constexpr int HH = HD / 2;
@@ -56,8 +69,66 @@ __device__ __forceinline__ void stage_row(T* tile, const T* base, long long st, 
   for (int g8 = 0; g8 < HH / 8; ++g8) {
     const int c = half * HH + g8 * 8;
     const bool in = tok >= 0 && c < D;
-    sm90::cp_async16(tile + sm90::core_off(row, c, HD), in ? src + c : base, in ? 16 : 0);
+    if constexpr (kSplit<T>) {
+      __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(tile) + sm90::core_off(row, c, HD);
+      sm90::cp_async16(hi, in ? src + c : base, in ? 16 : 0);
+      sm90::cp_async16(hi + 64 * HD, in ? src + c + 4 : base, in ? 16 : 0);
+    } else {
+      sm90::cp_async16(tile + sm90::core_off(row, c, HD), in ? src + c : base, in ? 16 : 0);
+    }
   }
+}
+
+// hi = bf16(x), lo = bf16(x - hi) of two values, packed as an A fragment register (x - hi is exact in fp32)
+__device__ __forceinline__ void split2(float x, float y, uint32_t& hi, uint32_t& lo) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = sm90::pack2<__nv_bfloat16>(x - __low2float(h), y - __high2float(h));
+}
+
+// Converts in place the row segment stage_row copied into a split fp32 tile (run by the thread that copied it, after its
+// copies have landed: it reads and writes only those bytes).  Zero-filled phantom rows and columns give hi = lo = 0.
+template <int HD>
+__device__ __forceinline__ void split_row(float* tile, int row, int half) {
+  constexpr int HH = HD / 2;
+#pragma unroll
+  for (int g8 = 0; g8 < HH / 8; ++g8) {
+    __nv_bfloat16* hp = reinterpret_cast<__nv_bfloat16*>(tile) + sm90::core_off(row, half * HH + g8 * 8, HD);
+    uint4* hi = reinterpret_cast<uint4*>(hp);
+    uint4* lo = reinterpret_cast<uint4*>(hp + 64 * HD);
+    const float4 x = *reinterpret_cast<const float4*>(hi), y = *reinterpret_cast<const float4*>(lo);
+    uint4 h, l;
+    split2(x.x, x.y, h.x, l.x);
+    split2(x.z, x.w, h.y, l.y);
+    split2(y.x, y.y, h.z, l.z);
+    split2(y.z, y.w, h.w, l.w);
+    *hi = h;
+    *lo = l;
+  }
+}
+
+// The two products the split adds to an SS product over HD: A_hi B_lo + A_lo B_hi (A, B: split fp32 tiles)
+template <int HD>
+__device__ __forceinline__ void split_ss(float (&d)[32], const float* A, const float* B) {
+  using W64 = sm90::Wg<__nv_bfloat16, 64>;
+  const __nv_bfloat16* a = reinterpret_cast<const __nv_bfloat16*>(A);
+  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(B);
+#pragma unroll
+  for (int kk = 0; kk < HD / 16; ++kk) W64::ss(d, sm90::desc(a, HD, kk), sm90::desc(b + 64 * HD, HD, kk), 1);
+#pragma unroll
+  for (int kk = 0; kk < HD / 16; ++kk) W64::ss(d, sm90::desc(a + 64 * HD, HD, kk), sm90::desc(b, HD, kk), 1);
+}
+
+// The two products the split adds to an RS product over the 64 columns of a piece: A_hi B_lo + A_lo B_hi (A: the hi /
+// lo fragments of an accumulator tile, B: a split fp32 tile read MN-major)
+template <int HD>
+__device__ __forceinline__ void split_rs(float (&d)[HD / 2], const uint32_t (&hi)[4][4], const uint32_t (&lo)[4][4], const float* B) {
+  using WHD = sm90::Wg<__nv_bfloat16, HD>;
+  const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(B);
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) WHD::rs(d, hi[kk], sm90::desc_mn(b + 64 * HD, HD, kk), 1);
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) WHD::rs(d, lo[kk], sm90::desc_mn(b, HD, kk), 1);
 }
 
 // A operand of the k16 slice kk from a 64-column accumulator tile
@@ -67,6 +138,20 @@ __device__ __forceinline__ void to_a_frag(const float (&s)[32], int kk, uint32_t
   a[1] = sm90::pack2<T>(s[8 * kk + 2], s[8 * kk + 3]);
   a[2] = sm90::pack2<T>(s[8 * kk + 4], s[8 * kk + 5]);
   a[3] = sm90::pack2<T>(s[8 * kk + 6], s[8 * kk + 7]);
+}
+
+// A operands of all four k16 slices of a 64-column accumulator tile; split: also the lo fragments
+template <typename T>
+__device__ __forceinline__ void to_a_frags(const float (&s)[32], uint32_t (&a)[4][4], uint32_t (&lo)[4][4]) {
+  if constexpr (kSplit<T>) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) split2(s[8 * kk + 2 * j], s[8 * kk + 2 * j + 1], a[kk][j], lo[kk][j]);
+  } else {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) to_a_frag<T>(s, kk, a[kk]);
+  }
 }
 
 // acc (64 x HD) rows -> global rows (only the first D columns)
@@ -302,7 +387,7 @@ __device__ __forceinline__ void dq_scores(float (&s)[32], const float (&dp)[32],
   }
 }
 
-// Shared memory of a CTA: the stationary tiles, kStages<HD> stages of two streamed tiles each, as many sets of per-column
+// Shared memory of a CTA: the stationary tiles, kRing<T, HD> stages of two streamed tiles each, as many sets of per-column
 // metadata, the visit list and the bias table.
 constexpr size_t kKeyCols = 64 * (4 + 4 + 2 + 2);
 constexpr size_t kQueryCols = 64 * (4 + 4 + 4 + 2 + 2 + 1);
@@ -319,31 +404,31 @@ __device__ __forceinline__ KeyCols key_cols(unsigned char* meta, int stage) {
   return kc;
 }
 
-template <int HD> struct FwdSmem {     // Q; K, V per stage
-  static constexpr size_t tiles = (1 + 2 * kStages<HD>) * 64 * HD * 2;
-  static size_t total(int tabn) { return (tiles + kStages<HD> * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
+template <typename T, int HD> struct FwdSmem {     // Q; K, V per stage
+  static constexpr size_t tiles = (1 + 2 * kRing<T, HD>) * 64 * HD * sizeof(T);
+  static size_t total(int tabn) { return (tiles + kRing<T, HD> * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15); }
 };
-template <int HD> struct DqSmem {      // Q, dO; K, V per stage; with the bias table, the dS tile after the table
-  static constexpr size_t tiles = (2 + 2 * kStages<HD>) * 64 * HD * 2;
+template <typename T, int HD> struct DqSmem {      // Q, dO; K, V per stage; with the bias table, the dS tile after the table
+  static constexpr size_t tiles = (2 + 2 * kRing<T, HD>) * 64 * HD * sizeof(T);
   static size_t total(int tabn, bool tab = false) {
-    return ((tiles + kStages<HD> * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15)) + (tab ? kDsTile : 0);
+    return ((tiles + kRing<T, HD> * kKeyCols + kVisits + (size_t)tabn * 4 + 15) & ~size_t(15)) + (tab ? kDsTile : 0);
   }
 };
-template <int HD> struct DkvSmem {     // K, V; Q, dO per stage; the key rows' chunk positions
-  static constexpr size_t tiles = (2 + 2 * kStages<HD>) * 64 * HD * 2;
+template <typename T, int HD> struct DkvSmem {     // K, V; Q, dO per stage; the key rows' chunk positions
+  static constexpr size_t tiles = (2 + 2 * kRing<T, HD>) * 64 * HD * sizeof(T);
   static size_t total(int tabn, bool drop = false) {
-    return (tiles + kStages<HD> * query_cols_bytes(drop) + kVisits + 64 * sizeof(int) + (size_t)tabn * 4 + 15) & ~size_t(15);
+    return (tiles + kRing<T, HD> * query_cols_bytes(drop) + kVisits + 64 * sizeof(int) + (size_t)tabn * 4 + 15) & ~size_t(15);
   }
 };
 
-// Stages key piece pi (K and V rows, the column metadata) into ring stage pi % kStages<HD> and commits it as one cp.async
+// Stages key piece pi (K and V rows, the column metadata) into ring stage pi % kRing<T, HD> and commits it as one cp.async
 // group; past the last piece it commits an empty group, so that every round waits on the same group count.
 template <typename T, int HD>
 __device__ __forceinline__ void issue_key_piece(const Geo& geo, int pi, int npieces, int ngp, const Visit* vl, SlotWalk& wk,
                                                 T* ring, unsigned char* meta, const T* kb, long long kst, const T* vb,
                                                 long long vst, int h, const float* __restrict__ g2l) {
   if (pi < npieces) {
-    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = pi % kStages<HD>;
+    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = pi % kRing<T, HD>;
     int gk, vr, vc;
     long long tok;
     bool ok;
@@ -357,10 +442,17 @@ __device__ __forceinline__ void issue_key_piece(const Geo& geo, int pi, int npie
 }
 
 // Top of round pi: piece pi has landed in every thread's copies, is visible to the async proxy, and every thread is done
-// with round pi - 1, whose stage the next issue refills.
-template <int HD>
-__device__ __forceinline__ void ring_wait() {
-  sm90::cp_async_wait<kStages<HD> - 2>();
+// with round pi - 1, whose stage the next issue refills.  Split fp32 tiles: before the barrier each thread converts the
+// rows it copied, those of the piece's two tiles at `piece` and in round 0 those of the n0 stationary tiles at `fixed`.
+template <typename T, int HD>
+__device__ __forceinline__ void ring_wait(T* piece, T* fixed, int n0) {
+  sm90::cp_async_wait<kRing<T, HD> - 2>();
+  if constexpr (kSplit<T>) {
+    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1;
+    split_row<HD>(piece, slot, half);
+    split_row<HD>(piece + 64 * HD, slot, half);
+    for (int i = 0; i < n0; ++i) split_row<HD>(fixed + i * 64 * HD, slot, half);
+  }
   sm90::fence_proxy_async();
   __syncthreads();
 }
@@ -369,19 +461,20 @@ __device__ __forceinline__ void ring_wait() {
 // forward, local queries
 // ----------------------------------------------------------------------------------------------
 // held to 5 / 3 CTAs per SM (HD <= 32 / 64): left alone, ptxas spends registers on hoisting the column loads and drops one.
-// HD 128: 2, what the 2-stage ring fits (the O accumulator alone is 64 registers)
+// HD 128: 2, what the 2-stage ring fits (the O accumulator alone is 64 registers).  Split fp32 tiles: 4 / 3 / 2 (HD 16 /
+// 32 / 64); at 5 the HD 16 kernel, with its lo fragments, spills.
 template <typename T, int HD, typename TO, bool DROP = false>
-__global__ void __launch_bounds__(kThreads, HD <= 32 ? 5 : HD <= 64 ? 3 : 2)
+__global__ void __launch_bounds__(kThreads, kSplit<T> ? (HD <= 16 ? 4 : HD <= 32 ? 3 : 2) : HD <= 32 ? 5 : HD <= 64 ? 3 : 2)
 wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const float* __restrict__ table,
              const float* __restrict__ g2l) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
-  using W64 = sm90::Wg<T, 64>;
-  using WHD = sm90::Wg<T, HD>;
+  using W64 = sm90::Wg<Op<T>, 64>;
+  using WHD = sm90::Wg<Op<T>, HD>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* Qs = reinterpret_cast<T*>(smem_raw);
   T* ring = Qs + TILE;                                            // stage s: K at ring + 2 s TILE, V after it
-  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages<HD> * TILE);
-  Visit* vl = reinterpret_cast<Visit*>(meta + kStages<HD> * kKeyCols);
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kRing<T, HD> * TILE);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kRing<T, HD> * kKeyCols);
   float* tab = reinterpret_cast<float*>(vl + 9);
   const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
 
@@ -408,12 +501,12 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   SlotWalk wk(geo, slot);
   __syncthreads();                                                // the visit list
 #pragma unroll
-  for (int p = 0; p < kStages<HD> - 1; ++p)                       // the first group also carries Q
+  for (int p = 0; p < kRing<T, HD> - 1; ++p)                       // the first group also carries Q
     issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
   for (int pi = 0; pi < npieces; ++pi) {
-    ring_wait<HD>();
-    issue_key_piece<T, HD>(geo, pi + kStages<HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
-    const int st = pi % kStages<HD>;
+    ring_wait<T, HD>(ring + pi % kRing<T, HD> * 2 * TILE, Qs, pi == 0 ? 1 : 0);
+    issue_key_piece<T, HD>(geo, pi + kRing<T, HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    const int st = pi % kRing<T, HD>;
     const T* Ks = ring + st * 2 * TILE;
     const T* Vs = Ks + TILE;
     const KeyCols kcol = key_cols(meta, st);
@@ -421,6 +514,7 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     sm90::wg_fence();
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk) W64::ss(s, sm90::desc(Qs, HD, kk), sm90::desc(Ks, HD, kk), kk > 0);
+    if constexpr (kSplit<T>) split_ss<HD>(s, Qs, Ks);
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(s);
@@ -457,12 +551,12 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
       drop_rows(geo, R, C, cid.piece, drow);
       drop_key_piece(s, geo, drow, drop_col_base(geo, vl, ngp, pi), 2u * (uint32_t)(b * geo.H + h), 1.f);
     }
-    uint32_t a[4][4];
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) to_a_frag<T>(s, kk, a[kk]);
+    uint32_t a[4][4], al[4][4];
+    to_a_frags<T>(s, a, al);
     sm90::wg_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) WHD::rs(oacc, a[kk], sm90::desc_mn(Vs, HD, kk), 1);
+    if constexpr (kSplit<T>) split_rs<HD>(oacc, a, al, Vs);
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(oacc);
@@ -488,18 +582,18 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
 // (vil_common.cuh: table_grad_piece).  Without TAB, one image per CTA and none of that code.
 // HD 128 is held to 2 CTAs per SM, what the 2-stage ring fits; below it ptxas is left alone.
 template <typename T, int HD, typename TO, bool DROP = false, bool TAB = false>
-__global__ void __launch_bounds__(kThreads, HD <= 64 ? 0 : 2)
+__global__ void __launch_bounds__(kThreads, kTileHD<T, HD> <= 64 ? 0 : 2)
 wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse, const float* __restrict__ delta,
           const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ tpart) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
-  using W64 = sm90::Wg<T, 64>;
-  using WHD = sm90::Wg<T, HD>;
+  using W64 = sm90::Wg<Op<T>, 64>;
+  using WHD = sm90::Wg<Op<T>, HD>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* Qs = reinterpret_cast<T*>(smem_raw);
   T* Gs = Qs + TILE;
   T* ring = Gs + TILE;                                            // stage s: K at ring + 2 s TILE, V after it
-  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages<HD> * TILE);
-  Visit* vl = reinterpret_cast<Visit*>(meta + kStages<HD> * kKeyCols);
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kRing<T, HD> * TILE);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kRing<T, HD> * kKeyCols);
   float* tab = reinterpret_cast<float*>(vl + 9);
   const int tabn = TAB ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
   float* dst = nullptr;                                           // TAB: the dS tile, 16-byte aligned after the table
@@ -548,12 +642,12 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   SlotWalk wk(geo, slot);
   __syncthreads();                                                // the visit list
 #pragma unroll
-  for (int p = 0; p < kStages<HD> - 1; ++p)                       // the first group also carries Q and dO
+  for (int p = 0; p < kRing<T, HD> - 1; ++p)                       // the first group also carries Q and dO
     issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
   for (int pi = 0; pi < npieces; ++pi) {
-    ring_wait<HD>();
-    issue_key_piece<T, HD>(geo, pi + kStages<HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
-    const int st = pi % kStages<HD>;
+    ring_wait<T, HD>(ring + pi % kRing<T, HD> * 2 * TILE, Qs, pi == 0 ? 2 : 0);
+    issue_key_piece<T, HD>(geo, pi + kRing<T, HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    const int st = pi % kRing<T, HD>;
     const T* Ks = ring + st * 2 * TILE;
     const T* Vs = Ks + TILE;
     const KeyCols kcol = key_cols(meta, st);
@@ -563,6 +657,10 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     for (int kk = 0; kk < HD / 16; ++kk) W64::ss(s, sm90::desc(Qs, HD, kk), sm90::desc(Ks, HD, kk), kk > 0);
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk) W64::ss(dp, sm90::desc(Gs, HD, kk), sm90::desc(Vs, HD, kk), kk > 0);
+    if constexpr (kSplit<T>) {
+      split_ss<HD>(s, Qs, Ks);
+      split_ss<HD>(dp, Gs, Vs);
+    }
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(s);
@@ -576,12 +674,12 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     // CTA-uniform: the bias-table forms run only in the TAB instantiation
     if (geo.exact == 1) dq_scores<TAB, true>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, dst);
     else dq_scores<TAB, false>(s, dp, geo, kcol, tab, qrow, gl, lse_r, del_r, dst);
-    uint32_t a[4][4];
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) to_a_frag<T>(s, kk, a[kk]);
+    uint32_t a[4][4], al[4][4];
+    to_a_frags<T>(s, a, al);
     sm90::wg_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) WHD::rs(dqacc, a[kk], sm90::desc_mn(Ks, HD, kk), 1);
+    if constexpr (kSplit<T>) split_rs<HD>(dqacc, a, al, Ks);
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(dqacc);
@@ -661,14 +759,14 @@ __device__ __forceinline__ QueryCols query_cols(unsigned char* meta, int stage, 
   return qc;
 }
 
-// Stages query piece qp (Q and dO rows, the column metadata with lse and delta) into ring stage qp % kStages<HD> and commits it
+// Stages query piece qp (Q and dO rows, the column metadata with lse and delta) into ring stage qp % kRing<T, HD> and commits it
 // as one cp.async group (an empty one past the last piece).  The walk runs over the chunks of vl, npc pieces each.
 template <typename T, int HD, bool DROP, typename Walk>
 __device__ __forceinline__ void issue_query_piece(const Geo& geo, int qp, int npieces, const Visit* vl, Walk& wk, T* ring,
                                                   unsigned char* meta, const T* qb, long long qst, const T* gb, long long gst,
                                                   const float* __restrict__ lse, const float* __restrict__ delta) {
   if (qp < npieces) {
-    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = qp % kStages<HD>, w = geo.w;
+    const int slot = threadIdx.x >> 1, half = threadIdx.x & 1, st = qp % kRing<T, HD>, w = geo.w;
     bool qv = false;
     long long tq = 0;
     int qa = 0, qb2 = 0, cut = 0;
@@ -737,21 +835,22 @@ __device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const
 }
 
 // held to 4 / 3 CTAs per SM (HD <= 32 / 64) without dropout, 3 / 2 with it: left alone, ptxas takes more registers and
-// fits one less.  HD 128: 2 with or without dropout, what the 2-stage ring fits.
+// fits one less.  HD 128: 2 with or without dropout, what the 2-stage ring fits.  Split fp32 tiles: 3 / 2 / 2 (HD 16 / 32
+// / 64): the hi and lo fragments of P and dS are 64 registers, and at one CTA more the HD 16 and HD 32 kernels spill.
 template <typename T, int HD, typename TO, bool DROP = false>
-__global__ void __launch_bounds__(kThreads, HD > 64 ? 2 : (HD <= 32 ? 4 : 3) - (DROP ? 1 : 0))
+__global__ void __launch_bounds__(kThreads, kSplit<T> ? (HD <= 16 ? 3 : 2) : HD > 64 ? 2 : (HD <= 32 ? 4 : 3) - (DROP ? 1 : 0))
 wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse, const float* __restrict__ delta,
            const float* __restrict__ table) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
-  using W64 = sm90::Wg<T, 64>;
-  using WHD = sm90::Wg<T, HD>;
+  using W64 = sm90::Wg<Op<T>, 64>;
+  using WHD = sm90::Wg<Op<T>, HD>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* Ks = reinterpret_cast<T*>(smem_raw);
   T* Vs = Ks + TILE;
   T* ring = Vs + TILE;                                            // stage s: Q at ring + 2 s TILE, dO after it
-  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kStages<HD> * TILE);
+  unsigned char* meta = reinterpret_cast<unsigned char*>(ring + 2 * kRing<T, HD> * TILE);
   const int cols = (int)query_cols_bytes(DROP);
-  Visit* vl = reinterpret_cast<Visit*>(meta + kStages<HD> * cols);
+  Visit* vl = reinterpret_cast<Visit*>(meta + kRing<T, HD> * cols);
   int* kpos = reinterpret_cast<int*>(vl + 9);
   float* tab = reinterpret_cast<float*>(kpos + 64);
   const int tw = 4 * geo.w - 1;
@@ -782,14 +881,14 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
   // dropout kernel at HD 32 a spill
   __syncthreads();                                                // the visit list, kpos
 #pragma unroll
-  for (int p = 0; p < kStages<HD> - 1; ++p)                       // the first group also carries K and V
+  for (int p = 0; p < kRing<T, HD> - 1; ++p)                       // the first group also carries K and V
     issue_query_piece<T, HD, DROP>(geo, p, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
                                    row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
   for (int qp = 0; qp < npieces; ++qp) {
-    ring_wait<HD>();
-    issue_query_piece<T, HD, DROP>(geo, qp + kStages<HD> - 1, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
+    ring_wait<T, HD>(ring + qp % kRing<T, HD> * 2 * TILE, Ks, qp == 0 ? 2 : 0);
+    issue_query_piece<T, HD, DROP>(geo, qp + kRing<T, HD> - 1, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
                                    row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
-    const int st = qp % kStages<HD>;
+    const int st = qp % kRing<T, HD>;
     const T* Qs = ring + st * 2 * TILE;
     const T* Gs = Qs + TILE;
     const QueryCols qcol = query_cols(meta, st, cols);
@@ -804,6 +903,10 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     for (int kk = 0; kk < HD / 16; ++kk) W64::ss(s, sm90::desc(Ks, HD, kk), sm90::desc(Qs, HD, kk), kk > 0);
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk) W64::ss(dp, sm90::desc(Vs, HD, kk), sm90::desc(Gs, HD, kk), kk > 0);
+    if constexpr (kSplit<T>) {
+      split_ss<HD>(s, Ks, Qs);
+      split_ss<HD>(dp, Vs, Gs);
+    }
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(s);
@@ -827,13 +930,26 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
       for (int i = 0; i < 32; ++i) s[i] = (keep >> i) & 1u ? s[i] * geo.drop_scale : 0.f;
     }
     uint32_t ap[4][4], ad[4][4];
+    if constexpr (kSplit<T>) {
+      uint32_t apl[4][4], adl[4][4];
+      to_a_frags<T>(s, ap, apl);
+      to_a_frags<T>(dp, ad, adl);
+      sm90::wg_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) { to_a_frag<T>(s, kk, ap[kk]); to_a_frag<T>(dp, kk, ad[kk]); }
-    sm90::wg_fence();
+      for (int kk = 0; kk < 4; ++kk) WHD::rs(dvacc, ap[kk], sm90::desc_mn(Gs, HD, kk), 1);
+      split_rs<HD>(dvacc, ap, apl, Gs);
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) WHD::rs(dvacc, ap[kk], sm90::desc_mn(Gs, HD, kk), 1);
+      for (int kk = 0; kk < 4; ++kk) WHD::rs(dkacc, ad[kk], sm90::desc_mn(Qs, HD, kk), 1);
+      split_rs<HD>(dkacc, ad, adl, Qs);
+    } else {
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) WHD::rs(dkacc, ad[kk], sm90::desc_mn(Qs, HD, kk), 1);
+      for (int kk = 0; kk < 4; ++kk) { to_a_frag<T>(s, kk, ap[kk]); to_a_frag<T>(dp, kk, ad[kk]); }
+      sm90::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) WHD::rs(dvacc, ap[kk], sm90::desc_mn(Gs, HD, kk), 1);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) WHD::rs(dkacc, ad[kk], sm90::desc_mn(Qs, HD, kk), 1);
+    }
     sm90::wg_commit();
     sm90::wg_wait0();
     sm90::reg_fence(dvacc);

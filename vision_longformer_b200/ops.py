@@ -7,6 +7,11 @@ consumes the outputs of the `query` / `kv` Linears *in place* (no transposes or
 .contiguous() copies, cf. longformer2d.py:126-149) and writes the attention
 output directly in (B, N, H*D) layout for `proj` (cf. :201-203).
 
+fp32 calls follow torch's fp32 matmul precision: when `torch.backends.cuda.matmul.fp32_precision` is "tf32" (after
+`torch.set_float32_matmul_precision("high")` or `("medium")`), `impl="auto"` and `impl="wgmma"` run fp32 on the wgmma
+tensor cores as split bf16 products (VIL_FLAG_F32_SPLIT, include/vil_attn.h); otherwise, and with `impl="simt"`, fp32
+runs on the SIMT family in full fp32.  The choice is made in the forward and reused by its backward.
+
 The backward is deterministic: identical inputs give bitwise-identical gradients on a given build and GPU model,
 including those of the relative-position-bias parameters (summed in a fixed order, no atomics), so it needs no special
 handling under torch.use_deterministic_algorithms(True).  The workspace is sized by vil_attn_workspace_bytes, which
@@ -75,6 +80,15 @@ def _base_params(q, k, nx, ny, w, nglo, exact, mode, scale, impl, skip_mask=0, f
     return p
 
 
+def _split_flag(x: torch.Tensor, impl: str) -> int:
+    """VIL_FLAG_F32_SPLIT for an fp32 call that may use the tensor cores: torch's fp32 matmul precision allows TF32 or
+    split-bf16 products.  `fp32_precision` is read rather than get_float32_matmul_precision() or matmul.allow_tf32,
+    which raise once the legacy and the new precision APIs have been mixed."""
+    if x.dtype != torch.float32 or impl == "simt":
+        return 0
+    return _lib.VIL_FLAG_F32_SPLIT if torch.backends.cuda.matmul.fp32_precision == "tf32" else 0
+
+
 def _dropout_state(device: torch.device, dropout_p: float):
     """(seed, offset) of one dropout forward, drawn from the default CUDA generator of `device` the way torch's own
     Philox-based kernels draw theirs: the generator's seed and its current offset, which is then advanced.  Host-side
@@ -105,7 +119,8 @@ def _workspace(p: VilAttnParams, backward: bool, device) -> torch.Tensor:
 def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx, ny, w, exact=0, mode=0,
                               scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0):
     """q:(B,H,Nloc,D) k,v:(B,H,N,D) qg:(B,H,g,D) kg,vg:(B,H,N,D) views; o/og preallocated output views.
-    `flags`: VIL_FLAG_* of include/vil_attn.h (F32_OUT = 1: o / og are fp32 tensors - the parity build).
+    `flags`: VIL_FLAG_* of include/vil_attn.h (F32_OUT = 1: o / og are fp32 tensors - the parity build; F32_SPLIT = 4:
+    fp32 operands on the wgmma tensor cores as split bf16 products).
     `dropout_p` > 0: attention dropout with the mask of (dropout_seed, dropout_offset) (include/vil_attn.h); the
     backward must be given the same three values.
     Returns (lse (B,H,Nloc) fp32, lse_g (B,H,g) fp32 or None)."""
@@ -193,11 +208,12 @@ class _VilAttention(torch.autograd.Function):
         o = _heads(out, H)[:, :, g:]
         og = _heads(out, H)[:, :, :g] if g > 0 else None
         seed, offset = _dropout_state(q_all.device, dropout_p)
+        flags = _split_flag(q_all, impl)
         lse, lse_g = vil_attention_raw_forward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, nx=nx, ny=ny, w=w,
-                                               exact=exact, mode=mode, scale=scale, impl=impl, dropout_p=dropout_p,
-                                               dropout_seed=seed, dropout_offset=offset)
+                                               exact=exact, mode=mode, scale=scale, impl=impl, flags=flags,
+                                               dropout_p=dropout_p, dropout_seed=seed, dropout_offset=offset)
         ctx.save_for_backward(q_all, kv, qg_all, kvg, table, g2l, g2g, out, lse, lse_g)
-        ctx.cfg = (H, nx, ny, w, g, exact, mode, scale, impl, shared)
+        ctx.cfg = (H, nx, ny, w, g, exact, mode, scale, impl, shared, flags)
         ctx.drop = (dropout_p, seed, offset)
         return out
 
@@ -205,7 +221,7 @@ class _VilAttention(torch.autograd.Function):
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, d_out):
         q_all, kv, qg_all, kvg, table, g2l, g2g, out, lse, lse_g = ctx.saved_tensors
-        H, nx, ny, w, g, exact, mode, scale, impl, shared = ctx.cfg
+        H, nx, ny, w, g, exact, mode, scale, impl, shared, flags = ctx.cfg
         dropout_p, seed, offset = ctx.drop
         d_out = d_out.contiguous()
         k, v = _heads(kv, H, 0, 2), _heads(kv, H, 1, 2)
@@ -237,8 +253,8 @@ class _VilAttention(torch.autograd.Function):
         d_g2g = torch.zeros_like(g2g32) if g2g32 is not None else None
         vil_attention_raw_backward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, lse, lse_g, d_o, d_og,
                                    dq, dk, dv, dqg, dkg, dvg, d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=exact,
-                                   mode=mode, scale=scale, impl=impl, dropout_p=dropout_p, dropout_seed=seed,
-                                   dropout_offset=offset)
+                                   mode=mode, scale=scale, impl=impl, flags=flags, dropout_p=dropout_p,
+                                   dropout_seed=seed, dropout_offset=offset)
         cast = lambda d, ref: None if d is None else d.to(ref.dtype)
         return (dq_all, dkv, dqg_all, dkvg, cast(d_tab, table) if table is not None else None,
                 cast(d_g2l, g2l) if g2l is not None else None, cast(d_g2g, g2g) if g2g is not None else None,
@@ -292,11 +308,12 @@ class _VilAttentionPacked(torch.autograd.Function):
         o = _heads(out, H)[:, :, g:]
         og = _heads(out, H)[:, :, :g] if g > 0 else None
         seed, offset = _dropout_state(qkv.device, dropout_p)
+        flags = _split_flag(qkv, "auto")
         lse, lse_g = vil_attention_raw_forward(q, k, v, qg, k if g > 0 else None, v if g > 0 else None, tab32, g2l32, g2g32, o, og,
-                                               nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale, dropout_p=dropout_p,
-                                               dropout_seed=seed, dropout_offset=offset)
+                                               nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale, flags=flags,
+                                               dropout_p=dropout_p, dropout_seed=seed, dropout_offset=offset)
         ctx.save_for_backward(qkv, table, g2l, g2g, out, lse, lse_g)
-        ctx.cfg = (H, nx, ny, w, g, scale)
+        ctx.cfg = (H, nx, ny, w, g, scale, flags)
         ctx.drop = (dropout_p, seed, offset)
         return out
 
@@ -304,7 +321,7 @@ class _VilAttentionPacked(torch.autograd.Function):
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, d_out):
         qkv, table, g2l, g2g, out, lse, lse_g = ctx.saved_tensors
-        H, nx, ny, w, g, scale = ctx.cfg
+        H, nx, ny, w, g, scale, flags = ctx.cfg
         dropout_p, seed, offset = ctx.drop
         B, N, C3 = qkv.shape
         C = C3 // 3
@@ -322,8 +339,8 @@ class _VilAttentionPacked(torch.autograd.Function):
         d_g2g = torch.zeros_like(g2g32) if g2g32 is not None else None
         kg, vg, dkg, dvg = (k, v, dk, dv) if g > 0 else (None, None, None, None)
         vil_attention_raw_backward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, lse, lse_g, d_o, d_og, dq, dk, dv, dqg, dkg, dvg,
-                                   d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale, dropout_p=dropout_p,
-                                   dropout_seed=seed, dropout_offset=offset)
+                                   d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=0, mode=0, scale=scale, flags=flags,
+                                   dropout_p=dropout_p, dropout_seed=seed, dropout_offset=offset)
         cast = lambda d, ref: None if (d is None or ref is None) else d.to(ref.dtype)
         return d_qkv, cast(d_tab, table), cast(d_g2l, g2l), cast(d_g2g, g2g), None, None, None, None, None, None, None
 
