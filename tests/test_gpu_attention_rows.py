@@ -186,6 +186,15 @@ def where_chunk(idx, nx, ny, w):
         b, h, R, C, mx, my, ", padded" if (R == mx - 1 and padx) or (C == my - 1 and pady) else "")
 
 
+def store_eps(variant):
+    """(eps, out_eps) of a variant's stored outputs: the unit roundoff of the o that delta is formed from (`peak_floors`),
+    and the rms of one rounding of a stored gradient row, which the global-query backward pays once per global query
+    (`check`).  Both are those of fp32 where the outputs are fp32."""
+    impl, dtype, f32out, layout = VARIANTS[variant]
+    low = dtype == BF16 and not f32out
+    return (2.0 ** -8 if low else 2.0 ** -24), (2.0 ** -9 if low else 0.0)
+
+
 def peak_floors(t, cfg, variant, g):
     """Floors for the gradients under a saturated softmax, where a reference row is tiny by construction.
 
@@ -202,7 +211,7 @@ def peak_floors(t, cfg, variant, g):
     """
     impl, dtype, f32out, layout = VARIANTS[variant]
     nx, ny, w, exact, mode, scale = cfg
-    eps = 2.0 ** -8 if (dtype == BF16 and not f32out) else 2.0 ** -24
+    eps = store_eps(variant)[0]
     tiny = 2.0 ** -24 if dtype == F16 else 2.0 ** -126      # P and dS below it are flushed to zero as tensor-core operands
     rn = lambda x: x.to(dtype).double().norm(dim=-1)
     nloc = nx * ny
@@ -264,7 +273,7 @@ def check(test, tag, out, ref, case, variant, floors=None, bias=True, backward=T
     # The global-query backward adds each global query's term into the stored dkg / dvg rows (dk / dv with shared global
     # weights): g successive roundings to the output type, 2^-9 sqrt(g) rms in bf16 (measured: 2.8e-3 sqrt(g) in the worst
     # row at g = 16, 64, 65, 130).  DESIGN.md section 3 has it as a known loss of the bf16 / fp16 outputs at large g.
-    out_eps = 2.0 ** -9 if (VARIANTS[variant][1] == BF16 and not VARIANTS[variant][2]) else 0.0
+    out_eps = store_eps(variant)[1]
     many = 3 * out_eps * g ** 0.5 if g >= 4 else 0.0
     shared = "dkg" not in ref
     rows("o.row", out["o"], ref["o"], rf)
