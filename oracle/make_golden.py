@@ -87,6 +87,15 @@ ATTN_CASES = {
     "w5_g0_exact0_rpe":      (1, 12, 13, dict(dim=16, num_heads=2, w=5, nglo=0, exact=0, rpe=True, sharew=False), None),
     "w8_g1_exact0_d32":      (1, 24, 16, dict(dim=64, num_heads=2, w=8, nglo=1, exact=0, rpe=False, sharew=True), None),
     "w7_g1_exact0_d64_28":   (1, 28, 28, dict(dim=64, num_heads=1, w=7, nglo=1, exact=0, rpe=True, sharew=True), None),
+    # cyclic chunks with a pinned draw: the neighbour above left wraps for the first chunk row and column
+    "w4_g1_cyclic_mode1_pad": (2, 10, 9, dict(dim=16, num_heads=2, w=4, nglo=1, exact=-1, rpe=True, sharew=True, mode=1), 1),
+    # one padded chunk: both offsets wrap onto it
+    "w4_g1_cyclic_1x1_mode8": (2, 3, 3, dict(dim=16, num_heads=2, w=4, nglo=1, exact=-1, rpe=True, sharew=True, mode=1), 8),
+    "w7_g1_exact1_5x3":      (2, 5, 3, dict(dim=16, num_heads=2, w=7, nglo=1, exact=1, rpe=True, sharew=True), None),
+    "w4_g1_exact0_1x9":      (2, 1, 9, dict(dim=16, num_heads=2, w=4, nglo=1, exact=0, rpe=True, sharew=True), None),
+    "w1_g1_exact0_7x6":      (2, 7, 6, dict(dim=16, num_heads=2, w=1, nglo=1, exact=0, rpe=True, sharew=True), None),
+    "w2_g1_exact1_5x7":      (2, 5, 7, dict(dim=16, num_heads=2, w=2, nglo=1, exact=1, rpe=True, sharew=True), None),
+    "w3_g1_cyclic_8x8":      (2, 8, 8, dict(dim=16, num_heads=2, w=3, nglo=1, exact=-1, rpe=True, sharew=True), None),
 }
 
 
