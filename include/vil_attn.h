@@ -80,7 +80,22 @@ enum {
      they cover the call and the SIMT family elsewhere; VIL_IMPL_WGMMA fails where they do not; VIL_IMPL_SIMT ignores the
      flag.  The backward must be given the flag of its forward.  The bit leaves VilAttnParams as it was, so the ABI version
      stays 3: a library that predates the flag refuses it as an unknown bit (VIL_E_BADARG) rather than misreading it. */
-  VIL_FLAG_F32_SPLIT = 4
+  VIL_FLAG_F32_SPLIT = 4,
+  /* dilated sliding-chunk attention: VilAttnParams.dilation = d >= 1 (else VIL_E_BADARG); without the flag the word is
+     ignored and d = 1.  With d > 1 the local tokens fall into the d^2 residue classes (a, b) in [0, d)^2 of (r mod d,
+     c mod d); class (a, b) is a sub-grid of ceil((nx - a) / d) x ceil((ny - b) / d) tokens whose token (r', c') is image
+     position (a + d r', b + d c') (an empty class has no tokens).  A local query's output, lse and gradients are exactly
+     those of this operator run on its own sub-grid: same w, exact, mode, scale, the same global keys and values and bias
+     table, the sub-grid's own padding, chunk grid and cyclic wrap.  So exact = 1 is the dilated window |dr|, |dc| <= w d
+     with dr = dc = 0 (mod d), the reach in image positions growing with d (the receptive-field meaning of dilation; a
+     window |dr|, |dc| <= w restricted to multiples of d would not widen it).  The bias table is indexed by offsets in
+     sub-grid units (its shape does not change), one call's mode applies to every sub-grid, and global query rows attend
+     to all N tokens independently of d.  Dropout: the row of a local query is its image-grid local token i, the column
+     that of the query's sub-grid (offset index oi, key lk of the sub-grid chunk).  d = 1 is the undilated operator bit
+     for bit.  Both kernel families cover dilated calls on the terms they cover undilated ones.  The bit and the word,
+     which was padding, leave VilAttnParams as it was, so the ABI version stays 3: a library that predates the flag refuses
+     it as an unknown bit (VIL_E_BADARG). */
+  VIL_FLAG_DILATED = 16
 };
 
 /* error codes */
@@ -142,7 +157,8 @@ typedef struct VilAttnParams {
   void*   workspace;       /* device scratch, >= vil_attn_workspace_bytes(), 256-byte aligned.  The backward keeps
                               delta = rowsum(dO * O) of the local and global rows there and, when bias_table != NULL,
                               the partial sums of the three bias gradients (a bounded set for the table: it does not
-                              grow with B; per image for g2l / g2g) */
+                              grow with B, and grows with the residue sub-grids of a dilated call; per image for
+                              g2l / g2g) */
   int64_t workspace_bytes;
 
   /* ---- attention dropout (nn.Dropout on the softmax probabilities, longformer2d.py:186, 224); ABI v3 ----
@@ -158,7 +174,7 @@ typedef struct VilAttnParams {
      A (query, key) pair the reference visits through two offsets is two columns with two draws.  lse / lse_g stay the
      undropped softmax's. */
   float    dropout_p;
-  uint32_t reserved2;
+  int32_t  dilation;       /* d with VIL_FLAG_DILATED (see there), ignored without it */
   uint64_t dropout_seed;
   uint64_t dropout_offset;
 } VilAttnParams;

@@ -18,7 +18,7 @@ VIL_F32, VIL_BF16, VIL_F16 = 0, 1, 2
 VIL_IMPL_AUTO, VIL_IMPL_SIMT, VIL_IMPL_WGMMA = 0, 1, 2
 VIL_E_BADARG, VIL_E_UNSUPPORTED, VIL_E_CUDA, VIL_E_WORKSPACE = -1, -2, -3, -4
 ABI_VERSION = 3
-VIL_FLAG_F32_OUT, VIL_FLAG_UNFUSED, VIL_FLAG_F32_SPLIT = 1, 2, 4
+VIL_FLAG_F32_OUT, VIL_FLAG_UNFUSED, VIL_FLAG_F32_SPLIT, VIL_FLAG_DILATED = 1, 2, 4, 16
 
 # every symbol include/vil_attn.h declares
 EXPORTS = (
@@ -52,7 +52,7 @@ class VilAttnParams(ctypes.Structure):
         ("dqg", VilTensor4), ("dkg", VilTensor4), ("dvg", VilTensor4),
         ("d_bias_table", ctypes.c_void_p), ("d_g2l", ctypes.c_void_p), ("d_g2g", ctypes.c_void_p),
         ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_int64),
-        ("dropout_p", ctypes.c_float), ("reserved2", ctypes.c_uint32),
+        ("dropout_p", ctypes.c_float), ("dilation", ctypes.c_int32),
         ("dropout_seed", ctypes.c_uint64), ("dropout_offset", ctypes.c_uint64),
     ]
 

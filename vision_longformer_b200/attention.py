@@ -71,7 +71,10 @@ class B200Long2DSCSelfAttention(nn.Module):
         self.attention_window = w
         self.attention_dilation = d
         self.autoregressive = autoregressive
-        assert self.attention_dilation == 1, "Dilation is not supported!"
+        # d > 1: dilated sliding chunks, each query attending within its residue sub-grid (ops.vil_attention); only_glo has
+        # no local window and ignores d
+        if int(d) != d or d < 1:
+            raise ValueError(f"dilation d must be an integer >= 1 (got {d})")
         assert not self.autoregressive, "Autoregressive is not supported yet!"
         if exact not in (0, 1, -1):
             raise ValueError("longsc exact should be in [0,1,-1]!")
@@ -139,7 +142,7 @@ class B200Long2DSCSelfAttention(nn.Module):
         g2l = self.g2l_relative_position_bias if (self.rpe and g >= 1) else None
         g2g = self.g2g_relative_position_bias if (self.rpe and g >= 1) else None
         kw = dict(num_heads=H, nx=nx, ny=ny, w=self.attention_window, nglo=g, exact=self.exact, mode=mode,
-                  scale=self.scale, impl=self.impl, dropout_p=drop)
+                  scale=self.scale, impl=self.impl, dropout_p=drop, dilation=int(self.attention_dilation))
         if g >= 1 and self.sharew:
             # one GEMM for local + global queries, the kv GEMM is not recomputed (cf. longformer2d.py:211)
             out = vil_attention(self._lin(self.query, x), self._lin(self.kv, x), None, None, table, g2l, g2g, **kw)

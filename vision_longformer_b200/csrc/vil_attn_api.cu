@@ -50,7 +50,10 @@ int make_geo(const VilAttnParams* p, vil::Geo* g) {
   if (p->exact != 0 && p->exact != 1 && p->exact != -1)
     return fail(VIL_E_BADARG, "longsc exact should be in [0,1,-1]!");
   if (p->mode < -1 || p->mode > 8) return fail(VIL_E_BADARG, "mode must be in [-1, 8]");
-  if (p->flags & ~(VIL_FLAG_F32_OUT | VIL_FLAG_UNFUSED | VIL_FLAG_F32_SPLIT)) return fail(VIL_E_BADARG, "unknown bits in flags");
+  if (p->flags & ~(VIL_FLAG_F32_OUT | VIL_FLAG_UNFUSED | VIL_FLAG_F32_SPLIT | VIL_FLAG_DILATED))
+    return fail(VIL_E_BADARG, "unknown bits in flags");
+  const int d = (p->flags & VIL_FLAG_DILATED) ? p->dilation : 1;
+  if (d < 1) return fail(VIL_E_BADARG, "dilation must be >= 1 with VIL_FLAG_DILATED (got %d)", p->dilation);
   if ((p->flags & VIL_FLAG_F32_OUT) && p->dtype == VIL_F32)
     return fail(VIL_E_BADARG, "VIL_FLAG_F32_OUT is the parity build of the bf16 / fp16 kernels; dtype is already fp32");
   if ((p->flags & VIL_FLAG_F32_SPLIT) && p->dtype != VIL_F32)
@@ -68,6 +71,12 @@ int make_geo(const VilAttnParams* p, vil::Geo* g) {
   g->pady = (p->w - p->ny % p->w) % p->w;
   g->mx = (p->nx + g->padx) / p->w;
   g->my = (p->ny + g->pady) / p->w;
+  g->d = d;
+  if (d > 1) {   // the virtual chunk grid of the d^2 residue sub-grids (vil_common.cuh, SubGrid): d x the largest one's
+    const int nx0 = (p->nx + d - 1) / d, ny0 = (p->ny + d - 1) / d;
+    g->mx = d * ((nx0 + p->w - 1) / p->w);
+    g->my = d * ((ny0 + p->w - 1) / p->w);
+  }
   g->Nloc = p->nx * p->ny;
   g->N = g->Nloc + p->nglo;
   g->w2 = p->w * p->w;

@@ -30,11 +30,88 @@ struct Geo {
   // with the bias table: backward pass 1 runs nslice * H * mx * my * npc CTAs, CTA slice s taking the images
   // s, s + nslice, ...; a function of the geometry and the SM count only, so the table partials do not grow with B
   int nslice;
+  // dilation (VIL_FLAG_DILATED): 1, or d > 1 for a call run by the DIL instantiations of the local kernels (SubGrid below).
+  // The field fills the struct's tail padding, so the kernel parameters after it keep their offsets.
+  int d;
 };
+
+// Dilated calls (d > 1) run the operator on each of the d^2 residue sub-grids of the image: residue (a, b) holds the local
+// tokens (a + d r, b + d c).  mx / my then count the chunks of a virtual grid of d mx0 x d my0 chunks (mx0 x my0: the chunk
+// grid of the largest sub-grid, residue (0, 0)); virtual chunk (R', C') is chunk (R' / d, C' / d) of residue
+// (R' % d, C' % d).  Every grid, CTA count and workspace size derived from mx / my thereby covers the d^2 sub-grids, and a
+// CTA whose chunk lies outside its (smaller) sub-grid exits.  SubGrid is the geometry a CTA's masks use: its sub-grid's
+// tokens, padding and chunk counts, and its residue; undilated, Geo's own.
+template <bool DIL> struct SubGrid;
+template <> struct SubGrid<true> {
+  int nx_, ny_, padx_, pady_, mx_, my_;
+  int r0_, c0_;         // residue (a, b)
+  __device__ __forceinline__ int nx() const { return nx_; }
+  __device__ __forceinline__ int ny() const { return ny_; }
+  __device__ __forceinline__ int padx() const { return padx_; }
+  __device__ __forceinline__ int pady() const { return pady_; }
+  __device__ __forceinline__ int mx() const { return mx_; }
+  __device__ __forceinline__ int my() const { return my_; }
+  __device__ __forceinline__ int r0() const { return r0_; }
+  __device__ __forceinline__ int c0() const { return c0_; }
+};
+// undilated: Geo's own fields.  The kernels read them through VIL_SG / VIL_SUB_* below, which compile to the direct reads
+// of Geo the undilated kernels have always made.
+template <> struct SubGrid<false> {
+  const Geo& g;
+  __device__ __forceinline__ int nx() const { return g.nx; }
+  __device__ __forceinline__ int ny() const { return g.ny; }
+  __device__ __forceinline__ int padx() const { return g.padx; }
+  __device__ __forceinline__ int pady() const { return g.pady; }
+  __device__ __forceinline__ int mx() const { return g.mx; }
+  __device__ __forceinline__ int my() const { return g.my; }
+  __device__ __forceinline__ int r0() const { return 0; }
+  __device__ __forceinline__ int c0() const { return 0; }
+};
+
+// The CTA's sub-grid; R, C: in the virtual chunk position, out the chunk position in the sub-grid
+template <bool DIL>
+__device__ __forceinline__ SubGrid<DIL> sub_grid(const Geo& g, int& R, int& C) {
+  if constexpr (DIL) {
+    SubGrid<true> s;
+    s.r0_ = R % g.d; R /= g.d;
+    s.c0_ = C % g.d; C /= g.d;
+    s.nx_ = (g.nx - s.r0_ + g.d - 1) / g.d;
+    s.ny_ = (g.ny - s.c0_ + g.d - 1) / g.d;
+    s.padx_ = (g.w - s.nx_ % g.w) % g.w;
+    s.pady_ = (g.w - s.ny_ % g.w) % g.w;
+    s.mx_ = (s.nx_ + s.padx_) / g.w;
+    s.my_ = (s.ny_ + s.pady_) / g.w;
+    return s;
+  } else {
+    return SubGrid<false>{g};
+  }
+}
+// Field f (nx, ny, padx, pady, mx, my) of the sub-grid sg of a kernel or helper with template flag DIL and Geo `geo`.
+// Undilated it is geo.f read where it is used, so that those instantiations compile to the code they had before dilation
+// (read through SubGrid<false>, the same values compile to differently scheduled code).
+#define VIL_SG(f) (DIL ? sg.f() : geo.f)
+
+// a CTA of a dilated call whose chunk lies outside its sub-grid (never one of an undilated call)
+template <bool DIL>
+__device__ __forceinline__ bool off_sub_grid(const SubGrid<DIL>& s, int R, int C) {
+  if constexpr (DIL) return R >= s.mx() || C >= s.my();
+  else return false;
+}
+
+// The one mapping from a sub-grid position (r, c) to the image (tokens (a + d r, b + d c)), in a kernel or helper with
+// template flag DIL, Geo `geo` and sub-grid `sg`: the local token (row of q, o, lse, delta, dq), the same as a 32-bit value
+// (dropout rows), and the key token (row of k, v, dk, dv, after the g global tokens).  Macros for the reason VIL_SG is
+// one: undilated they are the expressions the kernels had before dilation.
+#define VIL_SUB_TOK(r, c) \
+  (DIL ? (long long)(sg.r0() + geo.d * (r)) * geo.ny + (sg.c0() + geo.d * (c)) : (long long)(r) * geo.ny + (c))
+#define VIL_SUB_ROW(r, c) (DIL ? (sg.r0() + geo.d * (r)) * geo.ny + (sg.c0() + geo.d * (c)) : (r) * geo.ny + (c))
+#define VIL_SUB_KEY(r, c) \
+  (DIL ? geo.g + (long long)(sg.r0() + geo.d * (r)) * geo.ny + (sg.c0() + geo.d * (c)) : geo.g + (long long)(r) * geo.ny + (c))
 
 // backward workspace layout (floats), each part 64-float aligned:
 //   [delta (B*H*Nloc)] [delta_g (B*H*g)]
-//   with the bias table only: [table partials (nslice*H*mx*my*npc, (4w-1)^2): one row per pass-1 CTA]
+//   with the bias table only: [table partials (nslice*H*mx*my*npc, (4w-1)^2): one row per pass-1 CTA (dilated: of the
+//                              virtual chunk grid, a CTA off its sub-grid leaving a row of zeros)]
 //                             [global-bias partials: d_g2l[1] (B,H,g) | d_g2l[0] (B,H,g) | d_g2g (B,H,g,g)]
 inline long long ws_align(long long n) { return (n + 63) & ~63LL; }
 inline long long ws_off_delta_g(const Geo& g) { return ws_align((long long)g.B * g.H * g.Nloc); }

@@ -89,7 +89,8 @@ int simt_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
     return shared_fail(VIL_E_UNSUPPORTED, "attention dropout supports head dim <= 64");
   } else {
   constexpr int L = DROP && std::is_same<T, float>::value && HD > 64 ? 4 : 2;
-  const auto kernel = simt_fwd_local<T, HD, L, DROP>;
+  // a dilated call (g.d > 1) runs the DIL instantiation over the d^2 residue sub-grids (vil_common.cuh, SubGrid)
+  const auto kernel = g.d > 1 ? simt_fwd_local<T, HD, L, DROP, true> : simt_fwd_local<T, HD, L, DROP>;
   const size_t sm = simt_tile_smem(g, Tile<HD, L>::HS, false);
   int rc = set_smem(kernel, sm);
   if (rc) return rc;
@@ -108,7 +109,7 @@ int simt_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
 // backward pass 1; TAB (the bias table): nslice image slices per (head, chunk, piece), table partials into the workspace
 template <typename T, int HD, int L, bool DROP, bool TAB>
 int simt_dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
-  const auto kernel = simt_bwd_dq<T, HD, L, DROP, TAB>;
+  const auto kernel = g.d > 1 ? simt_bwd_dq<T, HD, L, DROP, TAB, true> : simt_bwd_dq<T, HD, L, DROP, TAB>;
   const size_t sm = simt_tile_smem(g, Tile<HD, L>::HS, false) + (TAB ? simt_ds_tile_bytes() : 0);
   int rc = set_smem(kernel, sm);
   if (rc) return rc;
@@ -129,7 +130,7 @@ int simt_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
     constexpr int L = std::is_same<T, float>::value && HD > 64 ? 4 : 2;
     int rc = (p->skip_mask & 8) ? VIL_OK : delta_t<T, T>(p, g, s);
     if (rc) return rc;
-    const auto dkv = simt_bwd_dkv<T, HD, L, DROP>;
+    const auto dkv = g.d > 1 ? simt_bwd_dkv<T, HD, L, DROP, true> : simt_bwd_dkv<T, HD, L, DROP>;
     const size_t sm2 = simt_tile_smem(g, Tile<HD, L>::HS, true);
     if ((rc = set_smem(dkv, sm2))) return rc;
     const long long blocks = (long long)g.B * g.H * g.mx * g.my * g.npc;

@@ -58,7 +58,7 @@ __device__ __forceinline__ ChunkId decode_block(const Geo& g, int bid) {
 // ----------------------------------------------------------------------------------------------
 // forward, local queries
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, int L, bool DROP>
+template <typename T, int HD, int L, bool DROP, bool DIL = false>
 __global__ void __launch_bounds__(64 * L, L == 4 ? 1 : 0)
 simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
                const float* __restrict__ table, const float* __restrict__ g2l) {
@@ -75,23 +75,26 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
   unsigned char* kfl = reinterpret_cast<unsigned char*>(kvc + 64);
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
+  const int b = cid.b, h = cid.h;
+  int R = cid.R, C = cid.C;
   const int tid = threadIdx.x, slot = tid >> (L / 2), part = tid & (L - 1);
   const int w = geo.w, D = geo.D;
 
   for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
+  const auto sg = sub_grid<DIL>(geo, R, C);
+  if (off_sub_grid<DIL>(sg, R, C)) return;
 
   const int l = cid.piece * 64 + slot;
   const int qr = l / w, qc = l % w;
   const int r = R * w + qr, c = C * w + qc;
-  const bool qvalid = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
+  const bool qvalid = (l < geo.w2) && (r < VIL_SG(nx)) && (c < VIL_SG(ny));
 
   float qh[HP], oh[HP];
 #pragma unroll
   for (int i = 0; i < HP; ++i) { qh[i] = 0.f; oh[i] = 0.f; }
-  if (qvalid) load_seg<T, HP>(row_ptr<T>(q, b, h, (long long)r * geo.ny + c), part * HP, D, qh);
+  if (qvalid) load_seg<T, HP>(row_ptr<T>(q, b, h, VIL_SUB_TOK(r, c)), part * HP, D, qh);
   float m = -INFINITY, lsum = 0.f;
-  const uint32_t drow = (uint32_t)(r * geo.ny + c), dsid = 2u * (uint32_t)(b * geo.H + h);   // dropout: row, stream 0
+  const uint32_t drow = (uint32_t)VIL_SUB_ROW(r, c), dsid = 2u * (uint32_t)(b * geo.H + h);   // dropout: row, stream 0
 
   const int ngp = (geo.g + 63) / 64;
   const int npieces = ngp + geo.noffs * geo.npc;
@@ -105,8 +108,8 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
       if (DROP) cbase = geo.g + oi * geo.w2 + kp * 64;
       dR = geo.offR[oi]; dC = geo.offC[oi];
       KR = R + dR; KC = C + dC;
-      if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
-      else if (KR < 0 || KR >= geo.mx || KC < 0 || KC >= geo.my) continue;   // CTA-uniform
+      if (geo.exact == -1) { KR = (KR + VIL_SG(mx)) % VIL_SG(mx); KC = (KC + VIL_SG(my)) % VIL_SG(my); }
+      else if (KR < 0 || KR >= VIL_SG(mx) || KC < 0 || KC >= VIL_SG(my)) continue;   // CTA-uniform
     }
     __syncthreads();
     {   // stage one piece of <=64 keys: lane `part` of a slot loads its HP channels of a row of K and V
@@ -122,13 +125,13 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
         if (lk < geo.w2) {
           const int kr = lk / w, kc = lk % w;
           const int ar = KR * w + kr, ac = KC * w + kc;
-          const bool real = (ar < geo.nx) && (ac < geo.ny);
+          const bool real = (ar < VIL_SG(nx)) && (ac < VIL_SG(ny));
           if (geo.exact == -1)
-            flag = !(((R + dR == geo.mx - 1) && (kr >= w - geo.padx)) ||
-                     ((C + dC == geo.my - 1) && (kc >= w - geo.pady)));
+            flag = !(((R + dR == VIL_SG(mx) - 1) && (kr >= w - VIL_SG(padx))) ||
+                     ((C + dC == VIL_SG(my) - 1) && (kc >= w - VIL_SG(pady))));
           else
             flag = real;
-          if (flag && real) tok = geo.g + (long long)ar * geo.ny + ac;   // phantom padding keys keep K=V=0
+          if (flag && real) tok = VIL_SUB_KEY(ar, ac);   // phantom padding keys keep K=V=0
           vr = dR * w + kr; vc = dC * w + kc;
         }
       }
@@ -184,7 +187,7 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
     const float inv = (lsum > 0.f ? 1.f / lsum : 0.f) * (DROP ? geo.drop_scale : 1.f);
 #pragma unroll
     for (int i = 0; i < HP; ++i) oh[i] *= inv;
-    const long long tokq = (long long)r * geo.ny + c;
+    const long long tokq = VIL_SUB_TOK(r, c);
     store_seg<T, HP>(row_ptr_w<T>(o, b, h, tokq), part * HP, D, oh);
     if (part == 0) lse[((long long)b * geo.H + h) * geo.Nloc + tokq] = m + logf(lsum);
   }
@@ -329,7 +332,7 @@ __global__ void simt_bwd_delta(Geo geo, T4 o, T4 d_o, T4 og, T4 d_og,
 constexpr int kSimtDsLd = 65;   // dS tile row stride: the 16 query slots of a warp write one column in distinct banks
 inline size_t simt_ds_tile_bytes() { return 64 * kSimtDsLd * sizeof(float); }
 
-template <typename T, int HD, int L, bool DROP, bool TAB>
+template <typename T, int HD, int L, bool DROP, bool TAB, bool DIL = false>
 __global__ void __launch_bounds__(64 * L, L == 4 ? 1 : (TAB && HD <= 8 ? 4 : 0))
 simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse,
             const float* __restrict__ delta, const float* __restrict__ table,
@@ -349,7 +352,8 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
   float* acc = nullptr;                                   // TAB: the CTA's row of table partials
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
-  const int h = cid.h, R = cid.R, C = cid.C;
+  const int h = cid.h;
+  int R = cid.R, C = cid.C;
   const int tid = threadIdx.x, slot = tid >> (L / 2), part = tid & (L - 1);
   const int w = geo.w, D = geo.D;
   for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
@@ -359,12 +363,14 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
     acc = tpart + (long long)blockIdx.x * tabn;
     for (int i = tid; i < tabn; i += 64 * L) acc[i] = 0.f;
   }
+  const auto sg = sub_grid<DIL>(geo, R, C);
+  if (off_sub_grid<DIL>(sg, R, C)) return;             // after zeroing its row of table partials
 
   const int l = cid.piece * 64 + slot;
   const int qr = l / w, qc = l % w;
   const int r = R * w + qr, c = C * w + qc;
-  const bool qvalid = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
-  const long long tokq = (long long)r * geo.ny + c;
+  const bool qvalid = (l < geo.w2) && (r < VIL_SG(nx)) && (c < VIL_SG(ny));
+  const long long tokq = VIL_SUB_TOK(r, c);
 
   const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
   for (int it = 0; it < nimg; ++it) {
@@ -393,8 +399,8 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
       if (DROP) cbase = geo.g + oi * geo.w2 + kp * 64;
       dR = geo.offR[oi]; dC = geo.offC[oi];
       KR = R + dR; KC = C + dC;
-      if (geo.exact == -1) { KR = (KR + geo.mx) % geo.mx; KC = (KC + geo.my) % geo.my; }
-      else if (KR < 0 || KR >= geo.mx || KC < 0 || KC >= geo.my) continue;   // CTA-uniform
+      if (geo.exact == -1) { KR = (KR + VIL_SG(mx)) % VIL_SG(mx); KC = (KC + VIL_SG(my)) % VIL_SG(my); }
+      else if (KR < 0 || KR >= VIL_SG(mx) || KC < 0 || KC >= VIL_SG(my)) continue;   // CTA-uniform
     }
     __syncthreads();
     {
@@ -410,13 +416,13 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
         if (lk < geo.w2) {
           const int kr = lk / w, kc = lk % w;
           const int ar = KR * w + kr, ac = KC * w + kc;
-          const bool real = (ar < geo.nx) && (ac < geo.ny);
+          const bool real = (ar < VIL_SG(nx)) && (ac < VIL_SG(ny));
           if (geo.exact == -1)
-            flag = !(((R + dR == geo.mx - 1) && (kr >= w - geo.padx)) ||
-                     ((C + dC == geo.my - 1) && (kc >= w - geo.pady)));
+            flag = !(((R + dR == VIL_SG(mx) - 1) && (kr >= w - VIL_SG(padx))) ||
+                     ((C + dC == VIL_SG(my) - 1) && (kc >= w - VIL_SG(pady))));
           else
             flag = real;
-          if (flag && real) tok = geo.g + (long long)ar * geo.ny + ac;   // phantom padding keys keep K=V=0
+          if (flag && real) tok = VIL_SUB_KEY(ar, ac);   // phantom padding keys keep K=V=0
           vr = dR * w + kr; vc = dC * w + kc;
         }
       }
@@ -486,7 +492,7 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
 // backward pass 2 (key-stationary): dk, dv of the LOCAL key rows.  CTA = one 64-key piece of one
 // key chunk; it walks the query chunks that visit it (the symmetric image of the offset list).
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, int L, bool DROP>
+template <typename T, int HD, int L, bool DROP, bool DIL = false>
 __global__ void __launch_bounds__(64 * L, L == 4 ? 1 : 0)
 simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
              const float* __restrict__ delta, const float* __restrict__ table) {
@@ -506,16 +512,19 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
   int* qtok = reinterpret_cast<int*>(qfl + 64);            // DROP only: the query token of each staged column
 
   const ChunkId cid = decode_block(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, KR = cid.R, KC = cid.C;
+  const int b = cid.b, h = cid.h;
+  int KR = cid.R, KC = cid.C;
   const int tid = threadIdx.x, slot = tid >> (L / 2), part = tid & (L - 1);
   const int w = geo.w, D = geo.D;
   for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
+  const auto sg = sub_grid<DIL>(geo, KR, KC);
+  if (off_sub_grid<DIL>(sg, KR, KC)) return;
 
   const int lk = cid.piece * 64 + slot;
   const int kr = lk / w, kc = lk % w;
   const int ar = KR * w + kr, ac = KC * w + kc;
-  const bool kreal = (lk < geo.w2) && (ar < geo.nx) && (ac < geo.ny);
-  const long long tokk = geo.g + (long long)ar * geo.ny + ac;
+  const bool kreal = (lk < geo.w2) && (ar < VIL_SG(nx)) && (ac < VIL_SG(ny));
+  const long long tokk = VIL_SUB_KEY(ar, ac);
 
   float kh[HP], vh[HP], dkh[HP], dvh[HP];
 #pragma unroll
@@ -528,13 +537,13 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
   for (int oi = 0; oi < geo.noffs; ++oi) {
     const int dR = geo.offR[oi], dC = geo.offC[oi];
     int QR = KR - dR, QC = KC - dC;
-    if (geo.exact == -1) { QR = (QR + geo.mx) % geo.mx; QC = (QC + geo.my) % geo.my; }
-    else if (QR < 0 || QR >= geo.mx || QC < 0 || QC >= geo.my) continue;
+    if (geo.exact == -1) { QR = (QR + VIL_SG(mx)) % VIL_SG(mx); QC = (QC + VIL_SG(my)) % VIL_SG(my); }
+    else if (QR < 0 || QR >= VIL_SG(mx) || QC < 0 || QC >= VIL_SG(my)) continue;
     // is this key visible from query chunk (QR,QC) through offset (dR,dC)?
     bool kvis = kreal;
     if (geo.exact == -1)
-      kvis = kreal && !(((QR + dR == geo.mx - 1) && (kr >= w - geo.padx)) ||
-                        ((QC + dC == geo.my - 1) && (kc >= w - geo.pady)));
+      kvis = kreal && !(((QR + dR == VIL_SG(mx) - 1) && (kr >= w - VIL_SG(padx))) ||
+                        ((QC + dC == VIL_SG(my) - 1) && (kc >= w - VIL_SG(pady))));
     const int vr = dR * w + kr, vc = dC * w + kc;
     for (int qp = 0; qp < geo.npc; ++qp) {
       __syncthreads();
@@ -545,9 +554,9 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
         const int l = qp * 64 + slot;
         const int qr = l / w, qc = l % w;
         const int r = QR * w + qr, c = QC * w + qc;
-        const bool qv = (l < geo.w2) && (r < geo.nx) && (c < geo.ny);
+        const bool qv = (l < geo.w2) && (r < VIL_SG(nx)) && (c < VIL_SG(ny));
         if (qv) {
-          const long long tq = (long long)r * geo.ny + c;
+          const long long tq = VIL_SUB_TOK(r, c);
           load_seg<T, HP>(row_ptr<T>(q, b, h, tq), part * HP, D, qq);
           load_seg<T, HP>(row_ptr<T>(d_o, b, h, tq), part * HP, D, gg);
           if (part == 0) {
@@ -560,7 +569,7 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
 #pragma unroll
         for (int i = 0; i < HP; ++i) { qd[i] = qq[i]; gd[i] = gg[i]; }
         if (part == 0) { qrs[slot] = (short)qr; qcs[slot] = (short)qc; qfl[slot] = (unsigned char)qv; }
-        if (DROP && part == 0) qtok[slot] = r * geo.ny + c;
+        if (DROP && part == 0) qtok[slot] = VIL_SUB_ROW(r, c);
       }
       __syncthreads();
       for (int i2 = 0; i2 < 64; ++i2) {

@@ -68,9 +68,10 @@ int forward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   int rc;
   if (!(p->skip_mask & 2)) {
     const size_t sm = wg::FwdSmem<T, HD>::total(table_floats(g));
-    if ((rc = set_smem(wg::wg_fwd_local<T, HD, TO, DROP>, sm))) return rc;
-    wg::wg_fwd_local<T, HD, TO, DROP><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse,
-                                                                            p->bias_table, p->g2l);
+    // a dilated call (g.d > 1) runs the DIL instantiation over the d^2 residue sub-grids (vil_common.cuh, SubGrid)
+    const auto kernel = g.d > 1 ? wg::wg_fwd_local<T, HD, TO, DROP, true> : wg::wg_fwd_local<T, HD, TO, DROP>;
+    if ((rc = set_smem(kernel, sm))) return rc;
+    kernel<<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse, p->bias_table, p->g2l);
     count_launch();
     if ((rc = launch_check("wgmma_fwd_local"))) return rc;
   }
@@ -83,9 +84,10 @@ template <typename T, int HD, typename TO, bool DROP, bool TAB>
 int dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   int rc;
   const size_t sm = wg::DqSmem<T, HD>::total(table_floats(g), TAB);
-  if ((rc = set_smem(wg::wg_bwd_dq<T, HD, TO, DROP, TAB>, sm))) return rc;
+  const auto kernel = g.d > 1 ? wg::wg_bwd_dq<T, HD, TO, DROP, TAB, true> : wg::wg_bwd_dq<T, HD, TO, DROP, TAB>;
+  if ((rc = set_smem(kernel, sm))) return rc;
   const long long ctas = TAB ? tab_ctas(g) : blocks(g);
-  wg::wg_bwd_dq<T, HD, TO, DROP, TAB><<<(unsigned)ctas, wg::kThreads, sm, s>>>(
+  kernel<<<(unsigned)ctas, wg::kThreads, sm, s>>>(
       g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse, ws_at(p, 0), p->bias_table, p->g2l,
       TAB ? ws_at(p, ws_off_tab(g)) : nullptr);
   count_launch();
@@ -103,9 +105,10 @@ int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
   }
   if (!(p->skip_mask & 4)) {
     const size_t sm = wg::DkvSmem<T, HD>::total(tabn, DROP);
-    if ((rc = set_smem(wg::wg_bwd_dkv<T, HD, TO, DROP>, sm))) return rc;
-    wg::wg_bwd_dkv<T, HD, TO, DROP><<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk),
-                                                                          t4(p->dv), p->lse, delta, p->bias_table);
+    const auto kernel = g.d > 1 ? wg::wg_bwd_dkv<T, HD, TO, DROP, true> : wg::wg_bwd_dkv<T, HD, TO, DROP>;
+    if ((rc = set_smem(kernel, sm))) return rc;
+    kernel<<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv), p->lse,
+                                                         delta, p->bias_table);
     count_launch();
     if ((rc = launch_check("wgmma_bwd_dkv"))) return rc;
   }

@@ -184,11 +184,13 @@ __device__ __forceinline__ void drop_key_piece(float (&x)[32], const Geo& geo, c
 }
 
 // local token of the thread's two tile rows (past the image: any value, those rows are dropped)
-__device__ __forceinline__ void drop_rows(const Geo& geo, int R, int C, int piece, uint32_t (&row)[2]) {
+template <bool DIL>
+__device__ __forceinline__ void drop_rows(const Geo& geo, const SubGrid<DIL>& sg, int R, int C, int piece, uint32_t (&row)[2]) {
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     const int l = piece * 64 + acc_row(2 * e);
-    row[e] = (uint32_t)((R * geo.w + l / geo.w) * geo.ny + C * geo.w + l % geo.w);
+    row[e] = DIL ? (uint32_t)VIL_SUB_ROW(R * geo.w + l / geo.w, C * geo.w + l % geo.w)
+                 : (uint32_t)((R * geo.w + l / geo.w) * geo.ny + C * geo.w + l % geo.w);
   }
 }
 
@@ -204,16 +206,18 @@ struct Visit {
   int oi;       // the offset's index in Geo::offR / offC (the reference's block order; dropout columns)
 };
 
-// sgn = +1: the key chunks seen by query chunk (R, C); sgn = -1: the query chunks that see key chunk (R, C)
-__device__ __forceinline__ int visit_list(const Geo& geo, int R, int C, int sgn, Visit* vl) {
+// sgn = +1: the key chunks seen by query chunk (R, C); sgn = -1: the query chunks that see key chunk (R, C).  Chunks of the
+// CTA's sub-grid sg.
+template <bool DIL>
+__device__ __forceinline__ int visit_list(const Geo& geo, const SubGrid<DIL>& sg, int R, int C, int sgn, Visit* vl) {
   int n = 0;
   for (int oi = 0; oi < geo.noffs; ++oi) {
     const int dR = geo.offR[oi], dC = geo.offC[oi];
     int r = R + sgn * dR, c = C + sgn * dC;
-    if (geo.exact == -1) { r = (r + geo.mx) % geo.mx; c = (c + geo.my) % geo.my; }
-    else if (r < 0 || r >= geo.mx || c < 0 || c >= geo.my) continue;
+    if (geo.exact == -1) { r = (r + VIL_SG(mx)) % VIL_SG(mx); c = (c + VIL_SG(my)) % VIL_SG(my); }
+    else if (r < 0 || r >= VIL_SG(mx) || c < 0 || c >= VIL_SG(my)) continue;
     const int qR = sgn > 0 ? R : r, qC = sgn > 0 ? C : c;
-    if (threadIdx.x == 0) vl[n] = Visit{r, c, dR, dC, (qR + dR == geo.mx - 1) | ((qC + dC == geo.my - 1) << 1), oi};
+    if (threadIdx.x == 0) vl[n] = Visit{r, c, dR, dC, (qR + dR == VIL_SG(mx) - 1) | ((qC + dC == VIL_SG(my) - 1) << 1), oi};
     ++n;
   }
   return n;
@@ -256,30 +260,33 @@ struct SlotWalkLean {
 
 // Key (kr, kc) (kr < w) of visited chunk v: the token (-1: a zero row), whether the column takes part at all (the pad-cut
 // rule folded in), and the key's (row, column) relative to the query chunk's origin -- the rules of simt_fwd_local.
-__device__ __forceinline__ void chunk_key(const Geo& geo, const Visit& v, int kr, int kc, long long& tok, bool& ok, int& vr, int& vc) {
+template <bool DIL>
+__device__ __forceinline__ void chunk_key(const Geo& geo, const SubGrid<DIL>& sg, const Visit& v, int kr, int kc, long long& tok, bool& ok,
+                                          int& vr, int& vc) {
   const int w = geo.w;
   const int ar = v.r * w + kr, ac = v.c * w + kc;
-  const bool real = (ar < geo.nx) && (ac < geo.ny);
+  const bool real = (ar < VIL_SG(nx)) && (ac < VIL_SG(ny));
   if (geo.exact == -1)
-    ok = !(((v.cut & 1) && (kr >= w - geo.padx)) || ((v.cut & 2) && (kc >= w - geo.pady)));
+    ok = !(((v.cut & 1) && (kr >= w - VIL_SG(padx))) || ((v.cut & 2) && (kc >= w - VIL_SG(pady))));
   else
     ok = real;
-  tok = (ok && real) ? geo.g + (long long)ar * geo.ny + ac : -1;   // phantom padding keys keep K = V = 0
+  tok = (ok && real) ? VIL_SUB_KEY(ar, ac) : -1;   // phantom padding keys keep K = V = 0
   vr = v.dR * w + kr; vc = v.dC * w + kc;
 }
 
 // Column slot of key piece pi (ngp pieces of global keys, then npc per visited chunk, taken in order: the chunk pieces
 // advance `wk`): gk = the global key (-1 for a local one or an empty slot), then as chunk_key.  Global keys sit at (0, 0),
 // which every query of the chunk sees under the exact window.
-__device__ __forceinline__ void key_slot(const Geo& geo, const Visit* vl, int ngp, int pi, int slot, SlotWalk& wk, int& gk,
-                                         long long& tok, bool& ok, int& vr, int& vc) {
+template <bool DIL>
+__device__ __forceinline__ void key_slot(const Geo& geo, const SubGrid<DIL>& sg, const Visit* vl, int ngp, int pi, int slot, SlotWalk& wk,
+                                         int& gk, long long& tok, bool& ok, int& vr, int& vc) {
   gk = -1; tok = -1; ok = false; vr = 0; vc = 0;
   if (pi < ngp) {
     const int t = pi * 64 + slot;
     if (t < geo.g) { gk = t; tok = t; ok = true; }
     return;
   }
-  if (wk.kr < geo.w) chunk_key(geo, vl[wk.vi], wk.kr, wk.kc, tok, ok, vr, vc);
+  if (wk.kr < geo.w) chunk_key<DIL>(geo, sg, vl[wk.vi], wk.kr, wk.kc, tok, ok, vr, vc);
   wk.next(geo);
 }
 
@@ -298,7 +305,8 @@ struct QRows {
   bool ok[2];
 };
 
-__device__ __forceinline__ QRows query_rows(const Geo& geo, int R, int C, int piece) {
+template <bool DIL>
+__device__ __forceinline__ QRows query_rows(const Geo& geo, const SubGrid<DIL>& sg, int R, int C, int piece) {
   QRows q;
   const int w = geo.w;
 #pragma unroll
@@ -306,7 +314,7 @@ __device__ __forceinline__ QRows query_rows(const Geo& geo, int R, int C, int pi
     const int l = piece * 64 + acc_row(2 * e);
     const bool in = l < geo.w2;
     q.qr[e] = in ? l / w : 0; q.qc[e] = in ? l % w : 0;
-    q.ok[e] = in && (R * w + q.qr[e] < geo.nx) && (C * w + q.qc[e] < geo.ny);
+    q.ok[e] = in && (R * w + q.qr[e] < VIL_SG(nx)) && (C * w + q.qc[e] < VIL_SG(ny));
   }
   return q;
 }
@@ -423,8 +431,8 @@ template <typename T, int HD> struct DkvSmem {     // K, V; Q, dO per stage; the
 
 // Stages key piece pi (K and V rows, the column metadata) into ring stage pi % kRing<T, HD> and commits it as one cp.async
 // group; past the last piece it commits an empty group, so that every round waits on the same group count.
-template <typename T, int HD>
-__device__ __forceinline__ void issue_key_piece(const Geo& geo, int pi, int npieces, int ngp, const Visit* vl, SlotWalk& wk,
+template <typename T, int HD, bool DIL>
+__device__ __forceinline__ void issue_key_piece(const Geo& geo, const SubGrid<DIL>& sg, int pi, int npieces, int ngp, const Visit* vl, SlotWalk& wk,
                                                 T* ring, unsigned char* meta, const T* kb, long long kst, const T* vb,
                                                 long long vst, int h, const float* __restrict__ g2l) {
   if (pi < npieces) {
@@ -432,7 +440,7 @@ __device__ __forceinline__ void issue_key_piece(const Geo& geo, int pi, int npie
     int gk, vr, vc;
     long long tok;
     bool ok;
-    key_slot(geo, vl, ngp, pi, slot, wk, gk, tok, ok, vr, vc);
+    key_slot<DIL>(geo, sg, vl, ngp, pi, slot, wk, gk, tok, ok, vr, vc);
     T* Ks = ring + st * 2 * 64 * HD;
     stage_row<T, HD>(Ks, kb, kst, tok, slot, half, geo.D);
     stage_row<T, HD>(Ks + 64 * HD, vb, vst, tok, slot, half, geo.D);
@@ -463,7 +471,7 @@ __device__ __forceinline__ void ring_wait(T* piece, T* fixed, int n0) {
 // held to 5 / 3 CTAs per SM (HD <= 32 / 64): left alone, ptxas spends registers on hoisting the column loads and drops one.
 // HD 128: 2, what the 2-stage ring fits (the O accumulator alone is 64 registers).  Split fp32 tiles: 4 / 3 / 2 (HD 16 /
 // 32 / 64); at 5 the HD 16 kernel, with its lo fragments, spills.
-template <typename T, int HD, typename TO, bool DROP = false>
+template <typename T, int HD, typename TO, bool DROP = false, bool DIL = false>
 __global__ void __launch_bounds__(kThreads, kSplit<T> ? (HD <= 16 ? 4 : HD <= 32 ? 3 : 2) : HD <= 32 ? 5 : HD <= 64 ? 3 : 2)
 wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const float* __restrict__ table,
              const float* __restrict__ g2l) {
@@ -479,22 +487,25 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   const int tabn = geo.has_bias ? (4 * geo.w - 1) * (4 * geo.w - 1) : 0;
 
   const Cta cid = decode(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, R = cid.R, C = cid.C;
+  const int b = cid.b, h = cid.h;
+  int R = cid.R, C = cid.C;
   const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
   const int w = geo.w, D = geo.D;
   for (int i = tid; i < tabn; i += kThreads) tab[i] = table[(long long)i * geo.H + h];
+  const auto sg = sub_grid<DIL>(geo, R, C);
+  if (off_sub_grid<DIL>(sg, R, C)) return;
   {
     const int l = cid.piece * 64 + slot;
     const int r = R * w + l / w, c = C * w + l % w;
-    const bool real = l < geo.w2 && r < geo.nx && c < geo.ny;
-    stage_row<T, HD>(Qs, row_ptr<T>(q, b, h, 0), q.st, real ? (long long)r * geo.ny + c : -1, slot, half, D);
+    const bool real = l < geo.w2 && r < VIL_SG(nx) && c < VIL_SG(ny);
+    stage_row<T, HD>(Qs, row_ptr<T>(q, b, h, 0), q.st, real ? VIL_SUB_TOK(r, c) : -1, slot, half, D);
   }
   float m[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
   float oacc[HH];
 #pragma unroll
   for (int i = 0; i < HH; ++i) oacc[i] = 0.f;
 
-  const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, R, C, 1, vl) * geo.npc;
+  const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, sg, R, C, 1, vl) * geo.npc;
   const int epi = key_epilogue(geo);
   const T* kb = row_ptr<T>(k, b, h, 0);
   const T* vb = row_ptr<T>(v, b, h, 0);
@@ -502,10 +513,10 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   __syncthreads();                                                // the visit list
 #pragma unroll
   for (int p = 0; p < kRing<T, HD> - 1; ++p)                       // the first group also carries Q
-    issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    issue_key_piece<T, HD, DIL>(geo, sg, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
   for (int pi = 0; pi < npieces; ++pi) {
     ring_wait<T, HD>(ring + pi % kRing<T, HD> * 2 * TILE, Qs, pi == 0 ? 1 : 0);
-    issue_key_piece<T, HD>(geo, pi + kRing<T, HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    issue_key_piece<T, HD, DIL>(geo, sg, pi + kRing<T, HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
     const int st = pi % kRing<T, HD>;
     const T* Ks = ring + st * 2 * TILE;
     const T* Vs = Ks + TILE;
@@ -522,10 +533,10 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     const int gl = geo.g - pi * 64;
     // the row coordinates are derived where they are used: kept live across the loop, they cost the HD 32 forward a spill
     switch (epi) {   // CTA-uniform
-      case 0: fwd_scores<false, false>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
-      case 1: fwd_scores<false, true>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
-      case 2: fwd_scores<true, false>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
-      default: fwd_scores<true, true>(s, mx, geo, kcol, tab, query_rows(geo, R, C, cid.piece), gl); break;
+      case 0: fwd_scores<false, false>(s, mx, geo, kcol, tab, query_rows(geo, sg, R, C, cid.piece), gl); break;
+      case 1: fwd_scores<false, true>(s, mx, geo, kcol, tab, query_rows(geo, sg, R, C, cid.piece), gl); break;
+      case 2: fwd_scores<true, false>(s, mx, geo, kcol, tab, query_rows(geo, sg, R, C, cid.piece), gl); break;
+      default: fwd_scores<true, true>(s, mx, geo, kcol, tab, query_rows(geo, sg, R, C, cid.piece), gl); break;
     }
     float corr[2];
 #pragma unroll
@@ -548,7 +559,7 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     for (int i = 0; i < HH; ++i) oacc[i] *= corr[(i >> 1) & 1];
     if constexpr (DROP) {    // lsum keeps the undropped P; P V takes P * keep, 1 / (1 - p) is applied by the final store
       uint32_t drow[2];
-      drop_rows(geo, R, C, cid.piece, drow);
+      drop_rows<DIL>(geo, sg, R, C, cid.piece, drow);
       drop_key_piece(s, geo, drow, drop_col_base(geo, vl, ngp, pi), 2u * (uint32_t)(b * geo.H + h), 1.f);
     }
     uint32_t a[4][4], al[4][4];
@@ -561,13 +572,13 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
     sm90::wg_wait0();
     sm90::reg_fence(oacc);
   }
-  const QRows qrow = query_rows(geo, R, C, cid.piece);
+  const QRows qrow = query_rows(geo, sg, R, C, cid.piece);
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     lsum[e] += __shfl_xor_sync(0xffffffffu, lsum[e], 1);
     lsum[e] += __shfl_xor_sync(0xffffffffu, lsum[e], 2);
     if (!qrow.ok[e]) continue;
-    const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
+    const long long tokq = VIL_SUB_TOK(R * w + qrow.qr[e], C * w + qrow.qc[e]);
     const float inv = lsum[e] > 0.f ? 1.f / lsum[e] : 0.f;
     store_rows<TO, HD>(oacc, e, row_ptr_w<TO>(o, b, h, tokq), D, DROP ? inv * geo.drop_scale : inv);
     if ((tid & 3) == 0) lse[((long long)b * geo.H + h) * geo.Nloc + tokq] = m[e] + logf(lsum[e]);
@@ -581,7 +592,7 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
 // after each chunk piece's dQ product its dS tile is added, in a fixed order, to the CTA's row of table partials tpart
 // (vil_common.cuh: table_grad_piece).  Without TAB, one image per CTA and none of that code.
 // HD 128 is held to 2 CTAs per SM, what the 2-stage ring fits; below it ptxas is left alone.
-template <typename T, int HD, typename TO, bool DROP = false, bool TAB = false>
+template <typename T, int HD, typename TO, bool DROP = false, bool TAB = false, bool DIL = false>
 __global__ void __launch_bounds__(kThreads, kTileHD<T, HD> <= 64 ? 0 : 2)
 wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse, const float* __restrict__ delta,
           const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ tpart) {
@@ -600,7 +611,8 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   float* acc = nullptr;                                           // TAB: the CTA's row of table partials
 
   const Cta cid = decode(geo, blockIdx.x);
-  const int h = cid.h, R = cid.R, C = cid.C;
+  const int h = cid.h;
+  int R = cid.R, C = cid.C;
   const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
   const int w = geo.w, D = geo.D;
   for (int i = tid; i < tabn; i += kThreads) tab[i] = table[(long long)i * geo.H + h];
@@ -609,6 +621,8 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     acc = tpart + (long long)blockIdx.x * tabn;
     for (int i = tid; i < tabn; i += kThreads) acc[i] = 0.f;
   }
+  const auto sg = sub_grid<DIL>(geo, R, C);
+  if (off_sub_grid<DIL>(sg, R, C)) return;                       // after zeroing its row of table partials
   const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
   for (int it = 0; it < nimg; ++it) {
   const int b = cid.b + it * geo.nslice;
@@ -617,17 +631,17 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
   {
     const int l = cid.piece * 64 + slot;
     const int r = R * w + l / w, c = C * w + l % w;
-    const long long tokq = (l < geo.w2 && r < geo.nx && c < geo.ny) ? (long long)r * geo.ny + c : -1;
+    const long long tokq = (l < geo.w2 && r < VIL_SG(nx) && c < VIL_SG(ny)) ? VIL_SUB_TOK(r, c) : -1;
     stage_row<T, HD>(Qs, row_ptr<T>(q, b, h, 0), q.st, tokq, slot, half, D);
     stage_row<T, HD>(Gs, row_ptr<T>(d_o, b, h, 0), d_o.st, tokq, slot, half, D);
   }
-  const QRows qrow = query_rows(geo, R, C, cid.piece);
+  const QRows qrow = query_rows(geo, sg, R, C, cid.piece);
   float lse_r[2], del_r[2];
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     lse_r[e] = INFINITY; del_r[e] = 0.f;
     if (qrow.ok[e]) {
-      const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
+      const long long tokq = VIL_SUB_TOK(R * w + qrow.qr[e], C * w + qrow.qc[e]);
       lse_r[e] = lse[bh * geo.Nloc + tokq];
       del_r[e] = delta[bh * geo.Nloc + tokq];
     }
@@ -636,17 +650,17 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
 #pragma unroll
   for (int i = 0; i < HH; ++i) dqacc[i] = 0.f;
 
-  const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, R, C, 1, vl) * geo.npc;
+  const int ngp = (geo.g + 63) / 64, npieces = ngp + visit_list(geo, sg, R, C, 1, vl) * geo.npc;
   const T* kb = row_ptr<T>(k, b, h, 0);
   const T* vb = row_ptr<T>(v, b, h, 0);
   SlotWalk wk(geo, slot);
   __syncthreads();                                                // the visit list
 #pragma unroll
   for (int p = 0; p < kRing<T, HD> - 1; ++p)                       // the first group also carries Q and dO
-    issue_key_piece<T, HD>(geo, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    issue_key_piece<T, HD, DIL>(geo, sg, p, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
   for (int pi = 0; pi < npieces; ++pi) {
     ring_wait<T, HD>(ring + pi % kRing<T, HD> * 2 * TILE, Qs, pi == 0 ? 2 : 0);
-    issue_key_piece<T, HD>(geo, pi + kRing<T, HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
+    issue_key_piece<T, HD, DIL>(geo, sg, pi + kRing<T, HD> - 1, npieces, ngp, vl, wk, ring, meta, kb, k.st, vb, v.st, h, g2l);
     const int st = pi % kRing<T, HD>;
     const T* Ks = ring + st * 2 * TILE;
     const T* Vs = Ks + TILE;
@@ -668,7 +682,7 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     const int gl = geo.g - pi * 64;
     if constexpr (DROP) {    // dS = P (dP keep / (1 - p) - delta)
       uint32_t drow[2];
-      drop_rows(geo, R, C, cid.piece, drow);
+      drop_rows<DIL>(geo, sg, R, C, cid.piece, drow);
       drop_key_piece(dp, geo, drow, drop_col_base(geo, vl, ngp, pi), 2u * (uint32_t)(b * geo.H + h), geo.drop_scale);
     }
     // CTA-uniform: the bias-table forms run only in the TAB instantiation
@@ -694,7 +708,7 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     if (!qrow.ok[e]) continue;
-    const long long tokq = (long long)(R * w + qrow.qr[e]) * geo.ny + (C * w + qrow.qc[e]);
+    const long long tokq = VIL_SUB_TOK(R * w + qrow.qr[e], C * w + qrow.qc[e]);
     store_rows<TO, HD>(dqacc, e, row_ptr_w<TO>(dq, b, h, tokq), D, geo.scale);
   }
   }
@@ -731,7 +745,8 @@ __device__ __forceinline__ int key_pos(const Geo& geo, int piece, int row) {
 }
 
 // The thread's two key rows, from the positions key_pos wrote to kpos[64]
-__device__ __forceinline__ KRows key_rows(const Geo& geo, int KR, int KC, const int* kpos) {
+template <bool DIL>
+__device__ __forceinline__ KRows key_rows(const Geo& geo, const SubGrid<DIL>& sg, int KR, int KC, const int* kpos) {
   KRows k;
   const int w = geo.w, tw = 4 * w - 1;
 #pragma unroll
@@ -739,9 +754,9 @@ __device__ __forceinline__ KRows key_rows(const Geo& geo, int KR, int KC, const 
     const int pos = kpos[acc_row(2 * e)];
     const bool in = pos >> 16;
     k.kr[e] = pos & 0xff; k.kc[e] = (pos >> 8) & 0xff;
-    k.real[e] = in && (KR * w + k.kr[e] < geo.nx) && (KC * w + k.kc[e] < geo.ny);
+    k.real[e] = in && (KR * w + k.kr[e] < VIL_SG(nx)) && (KC * w + k.kc[e] < VIL_SG(ny));
     k.tb[e] = k.kr[e] * tw + k.kc[e] - (2 * w - 1) * (tw + 1);
-    k.cut[e] = (k.kr[e] >= w - geo.padx) | ((k.kc[e] >= w - geo.pady) << 1);
+    k.cut[e] = (k.kr[e] >= w - VIL_SG(padx)) | ((k.kc[e] >= w - VIL_SG(pady)) << 1);
   }
   return k;
 }
@@ -761,8 +776,8 @@ __device__ __forceinline__ QueryCols query_cols(unsigned char* meta, int stage, 
 
 // Stages query piece qp (Q and dO rows, the column metadata with lse and delta) into ring stage qp % kRing<T, HD> and commits it
 // as one cp.async group (an empty one past the last piece).  The walk runs over the chunks of vl, npc pieces each.
-template <typename T, int HD, bool DROP, typename Walk>
-__device__ __forceinline__ void issue_query_piece(const Geo& geo, int qp, int npieces, const Visit* vl, Walk& wk, T* ring,
+template <typename T, int HD, bool DROP, bool DIL, typename Walk>
+__device__ __forceinline__ void issue_query_piece(const Geo& geo, const SubGrid<DIL>& sg, int qp, int npieces, const Visit* vl, Walk& wk, T* ring,
                                                   unsigned char* meta, const T* qb, long long qst, const T* gb, long long gst,
                                                   const float* __restrict__ lse, const float* __restrict__ delta) {
   if (qp < npieces) {
@@ -773,8 +788,8 @@ __device__ __forceinline__ void issue_query_piece(const Geo& geo, int qp, int np
     if (wk.kr < w) {
       const Visit vq = vl[wk.vi];
       const int r = vq.r * w + wk.kr, c = vq.c * w + wk.kc;
-      qv = (r < geo.nx) && (c < geo.ny);
-      tq = (long long)r * geo.ny + c;
+      qv = (r < VIL_SG(nx)) && (c < VIL_SG(ny));
+      tq = VIL_SUB_TOK(r, c);
       qa = wk.kr - vq.dR * w; qb2 = wk.kc - vq.dC * w; cut = vq.cut;
     }
     wk.next(geo);
@@ -837,7 +852,7 @@ __device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const
 // held to 4 / 3 CTAs per SM (HD <= 32 / 64) without dropout, 3 / 2 with it: left alone, ptxas takes more registers and
 // fits one less.  HD 128: 2 with or without dropout, what the 2-stage ring fits.  Split fp32 tiles: 3 / 2 / 2 (HD 16 / 32
 // / 64): the hi and lo fragments of P and dS are 64 registers, and at one CTA more the HD 16 and HD 32 kernels spill.
-template <typename T, int HD, typename TO, bool DROP = false>
+template <typename T, int HD, typename TO, bool DROP = false, bool DIL = false>
 __global__ void __launch_bounds__(kThreads, kSplit<T> ? (HD <= 16 ? 3 : 2) : HD > 64 ? 2 : (HD <= 32 ? 4 : 3) - (DROP ? 1 : 0))
 wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse, const float* __restrict__ delta,
            const float* __restrict__ table) {
@@ -857,15 +872,18 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
   const int tabn = geo.has_bias ? tw * tw : 0;
 
   const Cta cid = decode(geo, blockIdx.x);
-  const int b = cid.b, h = cid.h, KR = cid.R, KC = cid.C;
+  const int b = cid.b, h = cid.h;
+  int KR = cid.R, KC = cid.C;
   const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
   const int w = geo.w, D = geo.D;
   const long long bh = (long long)b * geo.H + h;
   for (int i = tid; i < tabn; i += kThreads) tab[i] = table[(long long)i * geo.H + h];
+  const auto sg = sub_grid<DIL>(geo, KR, KC);
+  if (off_sub_grid<DIL>(sg, KR, KC)) return;
   {
     const int lk = cid.piece * 64 + slot;
     const int ar = KR * w + lk / w, ac = KC * w + lk % w;
-    const long long tokk = (lk < geo.w2 && ar < geo.nx && ac < geo.ny) ? geo.g + (long long)ar * geo.ny + ac : -1;
+    const long long tokk = (lk < geo.w2 && ar < VIL_SG(nx) && ac < VIL_SG(ny)) ? VIL_SUB_KEY(ar, ac) : -1;
     stage_row<T, HD>(Ks, row_ptr<T>(k, b, h, 0), k.st, tokk, slot, half, D);
     stage_row<T, HD>(Vs, row_ptr<T>(v, b, h, 0), v.st, tokk, slot, half, D);
     if (half == 0) kpos[slot] = key_pos(geo, cid.piece, slot);
@@ -874,7 +892,7 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
 #pragma unroll
   for (int i = 0; i < HH; ++i) { dkacc[i] = 0.f; dvacc[i] = 0.f; }
 
-  const int npieces = visit_list(geo, KR, KC, -1, vl) * geo.npc;
+  const int npieces = visit_list(geo, sg, KR, KC, -1, vl) * geo.npc;
   const int epi = query_epilogue(geo);
   std::conditional_t<(HD > 64), SlotWalkLean, SlotWalk> wk(geo, slot);
   // the (b, h) slices of q, dO, lse and delta are recomputed at each issue: kept live across the loop, they cost the
@@ -882,11 +900,11 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
   __syncthreads();                                                // the visit list, kpos
 #pragma unroll
   for (int p = 0; p < kRing<T, HD> - 1; ++p)                       // the first group also carries K and V
-    issue_query_piece<T, HD, DROP>(geo, p, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
+    issue_query_piece<T, HD, DROP, DIL>(geo, sg, p, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
                                    row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
   for (int qp = 0; qp < npieces; ++qp) {
     ring_wait<T, HD>(ring + qp % kRing<T, HD> * 2 * TILE, Ks, qp == 0 ? 2 : 0);
-    issue_query_piece<T, HD, DROP>(geo, qp + kRing<T, HD> - 1, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
+    issue_query_piece<T, HD, DROP, DIL>(geo, sg, qp + kRing<T, HD> - 1, npieces, vl, wk, ring, meta, row_ptr<T>(q, b, h, 0), q.st,
                                    row_ptr<T>(d_o, b, h, 0), d_o.st, lse + bh * geo.Nloc, delta + bh * geo.Nloc);
     const int st = qp % kRing<T, HD>;
     const T* Qs = ring + st * 2 * TILE;
@@ -918,12 +936,12 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     }
     // the key rows are read from kpos where they are used: kept live across the loop, they cost the HD 32 kernel a spill
     switch (epi) {   // CTA-uniform
-      case 0: dkv_probs<false, 0>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
-      case 1: dkv_probs<false, 1>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
-      case 2: dkv_probs<false, 2>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
-      case 3: dkv_probs<true, 0>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
-      case 4: dkv_probs<true, 1>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
-      default: dkv_probs<true, 2>(s, dp, geo, qcol, tab, key_rows(geo, KR, KC, kpos)); break;
+      case 0: dkv_probs<false, 0>(s, dp, geo, qcol, tab, key_rows(geo, sg, KR, KC, kpos)); break;
+      case 1: dkv_probs<false, 1>(s, dp, geo, qcol, tab, key_rows(geo, sg, KR, KC, kpos)); break;
+      case 2: dkv_probs<false, 2>(s, dp, geo, qcol, tab, key_rows(geo, sg, KR, KC, kpos)); break;
+      case 3: dkv_probs<true, 0>(s, dp, geo, qcol, tab, key_rows(geo, sg, KR, KC, kpos)); break;
+      case 4: dkv_probs<true, 1>(s, dp, geo, qcol, tab, key_rows(geo, sg, KR, KC, kpos)); break;
+      default: dkv_probs<true, 2>(s, dp, geo, qcol, tab, key_rows(geo, sg, KR, KC, kpos)); break;
     }
     if constexpr (DROP) {
 #pragma unroll
@@ -955,11 +973,11 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
     sm90::reg_fence(dvacc);
     sm90::reg_fence(dkacc);
   }
-  const KRows krow = key_rows(geo, KR, KC, kpos);
+  const KRows krow = key_rows(geo, sg, KR, KC, kpos);
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     if (!krow.real[e]) continue;
-    const long long tokk = geo.g + (long long)(KR * w + krow.kr[e]) * geo.ny + (KC * w + krow.kc[e]);
+    const long long tokk = VIL_SUB_KEY(KR * w + krow.kr[e], KC * w + krow.kc[e]);
     store_rows<TO, HD>(dkacc, e, row_ptr_w<TO>(dk, b, h, tokk), D, geo.scale);
     store_rows<TO, HD>(dvacc, e, row_ptr_w<TO>(dv, b, h, tokk), D, 1.f);
   }

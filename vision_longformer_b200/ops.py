@@ -59,9 +59,11 @@ def _f32c(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
 
 
 def _base_params(q, k, nx, ny, w, nglo, exact, mode, scale, impl, skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0,
-                 dropout_offset=0) -> VilAttnParams:
+                 dropout_offset=0, dilation=1) -> VilAttnParams:
     if exact not in (0, 1, -1):
         raise ValueError("longsc exact should be in [0,1,-1]!")          # slidingchunk_2d.py:343
+    if int(dilation) != dilation or dilation < 1:
+        raise ValueError(f"dilation must be an integer >= 1 (got {dilation})")
     if exact == 1 and mode != 0:
         raise ValueError("exact sliding window (exact=1) only supports mode=0")
     if q.dtype not in _DTYPES:
@@ -75,6 +77,9 @@ def _base_params(q, k, nx, ny, w, nglo, exact, mode, scale, impl, skip_mask=0, f
     p.scale = float(scale)
     p.skip_mask = int(skip_mask)
     p.flags = int(flags)
+    if dilation > 1:                             # d = 1 leaves the flag clear: the undilated operator, bit for bit
+        p.flags |= _lib.VIL_FLAG_DILATED
+        p.dilation = int(dilation)
     p.dropout_p = float(dropout_p)
     p.dropout_seed, p.dropout_offset = int(dropout_seed), int(dropout_offset)
     return p
@@ -117,18 +122,22 @@ def _workspace(p: VilAttnParams, backward: bool, device) -> torch.Tensor:
 
 
 def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx, ny, w, exact=0, mode=0,
-                              scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0):
+                              scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0,
+                              dilation=1):
     """q:(B,H,Nloc,D) k,v:(B,H,N,D) qg:(B,H,g,D) kg,vg:(B,H,N,D) views; o/og preallocated output views.
     `flags`: VIL_FLAG_* of include/vil_attn.h (F32_OUT = 1: o / og are fp32 tensors - the parity build; F32_SPLIT = 4:
     fp32 operands on the wgmma tensor cores as split bf16 products).
     `dropout_p` > 0: attention dropout with the mask of (dropout_seed, dropout_offset) (include/vil_attn.h); the
     backward must be given the same three values.
+    `dilation` d > 1: dilated sliding-chunk attention (VIL_FLAG_DILATED, include/vil_attn.h): each local query attends
+    within its residue sub-grid of image positions (a + d r', b + d c'); the backward must be given the same d.
     Returns (lse (B,H,Nloc) fp32, lse_g (B,H,g) fp32 or None)."""
     _require_cuda(q, "q")
     B, H, Nloc, D = q.shape
     g = k.shape[2] - Nloc
     assert Nloc == nx * ny, "Global dimension does not match!"           # longformer2d.py:111
-    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset)
+    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset,
+                     dilation)
     lse = torch.empty(B, H, Nloc, dtype=torch.float32, device=q.device)
     lse_g = torch.empty(B, H, g, dtype=torch.float32, device=q.device) if g > 0 else None
     p.q, p.k, p.v, p.o = _t4(q), _t4(k), _t4(v), _t4(o)
@@ -146,11 +155,13 @@ def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx
 
 def vil_attention_raw_backward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, lse, lse_g, d_o, d_og,
                                dq, dk, dv, dqg, dkg, dvg, d_table, d_g2l, d_g2g, *, nx, ny, w, exact=0, mode=0,
-                               scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0):
+                               scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0,
+                               dilation=1):
     _require_cuda(q, "q")
     Nloc = q.shape[2]
     g = k.shape[2] - Nloc
-    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset)
+    p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset,
+                     dilation)
     p.q, p.k, p.v, p.o = _t4(q), _t4(k), _t4(v), _t4(o)
     p.d_o, p.dq, p.dk, p.dv = _t4(d_o), _t4(dq), _t4(dk), _t4(dv)
     if g > 0:
@@ -179,7 +190,7 @@ class _VilAttention(torch.autograd.Function):
     # `vil_attention` (not via cast_inputs, which would also round the fp32 bias tables to bf16).
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda")
-    def forward(ctx, q_all, kv, qg_all, kvg, table, g2l, g2g, H, nx, ny, w, nglo, exact, mode, scale, impl, dropout_p):
+    def forward(ctx, q_all, kv, qg_all, kvg, table, g2l, g2g, H, nx, ny, w, nglo, exact, mode, scale, impl, dropout_p, dilation):
         _require_cuda(q_all, "q")
         B = q_all.shape[0]
         C = q_all.shape[2]
@@ -211,9 +222,10 @@ class _VilAttention(torch.autograd.Function):
         flags = _split_flag(q_all, impl)
         lse, lse_g = vil_attention_raw_forward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, nx=nx, ny=ny, w=w,
                                                exact=exact, mode=mode, scale=scale, impl=impl, flags=flags,
-                                               dropout_p=dropout_p, dropout_seed=seed, dropout_offset=offset)
+                                               dropout_p=dropout_p, dropout_seed=seed, dropout_offset=offset,
+                                               dilation=dilation)
         ctx.save_for_backward(q_all, kv, qg_all, kvg, table, g2l, g2g, out, lse, lse_g)
-        ctx.cfg = (H, nx, ny, w, g, exact, mode, scale, impl, shared, flags)
+        ctx.cfg = (H, nx, ny, w, g, exact, mode, scale, impl, shared, flags, dilation)
         ctx.drop = (dropout_p, seed, offset)
         return out
 
@@ -221,7 +233,7 @@ class _VilAttention(torch.autograd.Function):
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, d_out):
         q_all, kv, qg_all, kvg, table, g2l, g2g, out, lse, lse_g = ctx.saved_tensors
-        H, nx, ny, w, g, exact, mode, scale, impl, shared, flags = ctx.cfg
+        H, nx, ny, w, g, exact, mode, scale, impl, shared, flags, dilation = ctx.cfg
         dropout_p, seed, offset = ctx.drop
         d_out = d_out.contiguous()
         k, v = _heads(kv, H, 0, 2), _heads(kv, H, 1, 2)
@@ -254,15 +266,15 @@ class _VilAttention(torch.autograd.Function):
         vil_attention_raw_backward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, lse, lse_g, d_o, d_og,
                                    dq, dk, dv, dqg, dkg, dvg, d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=exact,
                                    mode=mode, scale=scale, impl=impl, flags=flags, dropout_p=dropout_p,
-                                   dropout_seed=seed, dropout_offset=offset)
+                                   dropout_seed=seed, dropout_offset=offset, dilation=dilation)
         cast = lambda d, ref: None if d is None else d.to(ref.dtype)
         return (dq_all, dkv, dqg_all, dkvg, cast(d_tab, table) if table is not None else None,
                 cast(d_g2l, g2l) if g2l is not None else None, cast(d_g2g, g2g) if g2g is not None else None,
-                None, None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None, None, None)
 
 
 def vil_attention(q_all, kv, qg_all=None, kvg=None, table=None, g2l=None, g2g=None, *, num_heads, nx, ny, w,
-                  nglo, exact=0, mode=0, scale=1.0, impl="auto", dropout_p=0.0):
+                  nglo, exact=0, mode=0, scale=1.0, impl="auto", dropout_p=0.0, dilation=1):
     """Fused local+global Vision-Longformer attention.
 
     shared weights (sharew):   q_all (B, nglo+nx*ny, C) = query(x);          kv (B, N, 2C) = kv(x)
@@ -276,13 +288,18 @@ def vil_attention(q_all, kv, qg_all=None, kvg=None, table=None, g2l=None, g2g=No
 
     `dropout_p` in [0, 1): attention dropout on the probabilities (the reference's `attn_drop`, longformer2d.py:186, 224).
     Each call draws a fresh mask from the device's default CUDA generator; the backward reuses it.
+
+    `dilation` d >= 1: dilated sliding-chunk attention.  The local tokens fall into d^2 residue sub-grids (image rows and
+    columns congruent mod d); each local query attends to the global tokens and, with the same w / exact / mode / bias
+    table, to the keys of its own sub-grid, so its window reaches w * d image positions.  Global queries are unchanged.
+    d = 1 is the undilated operator, bit for bit.
     """
     if q_all.is_cuda and torch.is_autocast_enabled("cuda"):
         dt = torch.get_autocast_dtype("cuda")
         cast = lambda t: t if (t is None or t.dtype == dt) else t.to(dt)
         q_all, kv, qg_all, kvg = cast(q_all), cast(kv), cast(qg_all), cast(kvg)
     return _VilAttention.apply(q_all, kv, qg_all, kvg, table, g2l, g2g, num_heads, nx, ny, w, nglo, exact, mode,
-                               float(scale), impl, float(dropout_p))
+                               float(scale), impl, float(dropout_p), int(dilation))
 
 
 class _VilAttentionPacked(torch.autograd.Function):
