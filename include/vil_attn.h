@@ -208,6 +208,30 @@ int vil_attn_fwd_sm100(const VilAttnParams* p, void* stream);
    and then added into d_bias_table / d_g2l / d_g2g. */
 int vil_attn_bwd_sm100(const VilAttnParams* p, void* stream);
 
+/* Per-image token grids in a padded batch (detection-style batches of images of different sizes padded to one extent).
+   image_hw: DEVICE array of B (h, w) int32 pairs; NULL -> VIL_E_BADARG.  The tensors keep the padded layout: local token
+   r*ny + c is still position (r, c) of the nx x ny grid.  Image b's grid is its top-left h_b x w_b tokens (1 <= h_b <= nx,
+   1 <= w_b <= ny); the other local tokens of image b are off-image.
+     - A local query on image b gets exactly the result of the unsized call on image b alone cropped to h_b x w_b: output,
+       lse and gradients under the same w, exact, mode, scale, bias table and global tokens, with the crop's own padding,
+       chunk grid and cyclic wrap (exact = -1 wraps around the image, not around the padded grid).
+     - A global query of image b attends to the nglo global keys and to image b's on-image local keys only (again the
+       cropped call), and the global keys' gradients collect only on-image queries.
+     - Off-image rows: o, dq, dk, dv (and dkg, dvg with separate global weights) are written as exact zeros, lse as -inf
+       (an empty softmax); every row is still written.  q, k, v, d_o (and kg, vg) at off-image tokens are never read, so
+       their contents, NaN or inf included, do not reach any output.
+     - Dilation composes: with VIL_FLAG_DILATED the d^2 residue sub-grids are those of the h_b x w_b crop.
+     - Dropout keeps its mask definition: a local query's row is its padded-grid local token i, its column comes from the
+       image's own chunk offsets (as in the dilated case); a global row's column is key token j in [0, N).
+     - Everything else (flags, dilation, dropout, impl, skip_mask, workspace size) is as for vil_attn_fwd_sm100 /
+       vil_attn_bwd_sm100; the workspace does not depend on the sizes.  With every image at (nx, ny) the result is bit for
+       bit that of the unsized entry point.
+   The host cannot read device memory without a synchronise, so the kernels clamp each entry to [1, nx] x [1, ny]: a bad
+   entry gives the result of the clamped size, never an out-of-bounds access.  Each sized call adds one launch that writes
+   the off-image rows. */
+int vil_attn_fwd_sized_sm100(const VilAttnParams* p, const int32_t* image_hw, void* stream);
+int vil_attn_bwd_sized_sm100(const VilAttnParams* p, const int32_t* image_hw, void* stream);
+
 /*
  * LayerNorm over the last dimension of a contiguous (rows, C) token stream - SURVEY.md section 8 (f) row 4, the
  * `norm` in front of the attention / MLP of AttnBlock and MlpBlock (src/models/msvit.py:256, 313-316, 327, 337-339).

@@ -24,6 +24,7 @@ VIL_FLAG_F32_OUT, VIL_FLAG_UNFUSED, VIL_FLAG_F32_SPLIT, VIL_FLAG_DILATED = 1, 2,
 EXPORTS = (
     "vil_attn_abi_version", "vil_attn_last_error", "vil_attn_launch_count", "vil_attn_last_impl", "vil_attn_last_kernel",
     "vil_attn_workspace_bytes", "vil_attn_wgmma_supported", "vil_attn_fwd_sm100", "vil_attn_bwd_sm100",
+    "vil_attn_fwd_sized_sm100", "vil_attn_bwd_sized_sm100",
     "vil_layernorm_workspace_bytes", "vil_layernorm_fwd_sm100", "vil_layernorm_bwd_sm100",
     "vil_addnorm_workspace_bytes", "vil_addnorm_fwd_sm100", "vil_addnorm_bwd_sm100",
     "vil_bias_act_workspace_bytes", "vil_bias_act_fwd_sm100", "vil_bias_act_bwd_sm100",
@@ -118,6 +119,9 @@ def load() -> ctypes.CDLL:
         for fn in (lib.vil_attn_fwd_sm100, lib.vil_attn_bwd_sm100):
             fn.restype = ctypes.c_int
             fn.argtypes = [ctypes.POINTER(VilAttnParams), ctypes.c_void_p]
+        for fn in (lib.vil_attn_fwd_sized_sm100, lib.vil_attn_bwd_sized_sm100):
+            fn.restype = ctypes.c_int
+            fn.argtypes = [ctypes.POINTER(VilAttnParams), ctypes.c_void_p, ctypes.c_void_p]
         lib.vil_layernorm_workspace_bytes.restype = ctypes.c_int64
         lib.vil_layernorm_workspace_bytes.argtypes = [ctypes.POINTER(VilLayerNormParams)]
         for fn in (lib.vil_layernorm_fwd_sm100, lib.vil_layernorm_bwd_sm100):

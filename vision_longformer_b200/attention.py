@@ -21,7 +21,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .ops import vil_attention
+from .ops import image_sizes_device, vil_attention
 
 
 def relative_position_index(w: int) -> torch.Tensor:
@@ -111,14 +111,16 @@ class B200Long2DSCSelfAttention(nn.Module):
         from .epilogue import linear_colsum_bias
         return linear_colsum_bias(x, layer.weight, layer.bias)
 
-    def forward(self, x, nx, ny, defer_proj_bias: bool = False):
+    def forward(self, x, nx, ny, defer_proj_bias: bool = False, image_sizes=None):
         """`defer_proj_bias=True` (used by the fused residual epilogue of the harness, SURVEY.md section 8 (f) row 4) returns
         `(out, bias)`: the output projection WITHOUT its bias plus the bias that the caller's residual-add kernel applies
-        (`bias` is None when nothing was deferred and `out` is complete).  The default is the reference's contract."""
+        (`bias` is None when nothing was deferred and `out` is complete).  The default is the reference's contract.
+        `image_sizes`: per-image token grids of a padded batch, host data of B (h, w) (ops.vil_attention); the rows of
+        off-image tokens come out as the projection of a zero attention output."""
         if defer_proj_bias:
             can = (not self.only_glo) and (self.Nglo == 0 or self.sharew) and not (self.training and self.proj_drop.p > 0)
             if not can:
-                return self.forward(x, nx, ny), None
+                return self.forward(x, nx, ny, image_sizes=image_sizes), None
         B, N, C = x.shape
         Nloc = nx * ny
         g, H = self.Nglo, self.num_heads
@@ -127,7 +129,7 @@ class B200Long2DSCSelfAttention(nn.Module):
             raise RuntimeError("B200Long2DSCSelfAttention only runs on a CUDA (sm_90a) device; there is no CPU "
                                "fallback (use the reference module / oracle for CPU parity checks)")
         if self.only_glo:
-            return self._forward_only_glo(x, nx, ny)
+            return self._forward_only_glo(x, nx, ny, image_sizes)
         mode = self._pick_mode()
         drop = self.attn_drop.p if self.training else 0.0
         if drop >= 1.0:
@@ -142,7 +144,8 @@ class B200Long2DSCSelfAttention(nn.Module):
         g2l = self.g2l_relative_position_bias if (self.rpe and g >= 1) else None
         g2g = self.g2g_relative_position_bias if (self.rpe and g >= 1) else None
         kw = dict(num_heads=H, nx=nx, ny=ny, w=self.attention_window, nglo=g, exact=self.exact, mode=mode,
-                  scale=self.scale, impl=self.impl, dropout_p=drop, dilation=int(self.attention_dilation))
+                  scale=self.scale, impl=self.impl, dropout_p=drop, dilation=int(self.attention_dilation),
+                  image_sizes=image_sizes)
         if g >= 1 and self.sharew:
             # one GEMM for local + global queries, the kv GEMM is not recomputed (cf. longformer2d.py:211)
             out = vil_attention(self._lin(self.query, x), self._lin(self.kv, x), None, None, table, g2l, g2g, **kw)
@@ -160,23 +163,37 @@ class B200Long2DSCSelfAttention(nn.Module):
             return F.linear(out, self.proj.weight), self.proj.bias
         return self.proj_drop(self.proj(out))
 
-    def _forward_only_glo(self, x, nx, ny):
+    def _forward_only_glo(self, x, nx, ny, image_sizes=None):
         """ONLY_GLOBAL ablation (longformer2d.py:130-132,189-192): local queries attend to the global tokens
-        only.  Not on the north-star path; plain PyTorch, kept for API completeness."""
+        only.  Not on the north-star path; plain PyTorch, kept for API completeness.  With `image_sizes` the global
+        queries' softmax leaves out the off-image keys and the off-image local rows are zero before `proj`; the input rows
+        of off-image tokens are replaced by zeros first, so that whatever they hold cannot reach an output or a gradient."""
         B, N, C = x.shape
         g, H, M = self.Nglo, self.num_heads, self.head_dim
+        hw = image_sizes_device(image_sizes, B, nx, ny, x.device)
+        keep = None
+        if hw is not None:    # (B, nx * ny) on-image local tokens
+            keep = ((torch.arange(nx, device=x.device)[None, :, None] < hw[:, 0, None, None]) &
+                    (torch.arange(ny, device=x.device)[None, None, :] < hw[:, 1, None, None])).reshape(B, nx * ny)
+            x = torch.cat([x[:, :g], torch.where(keep[:, :, None], x[:, g:], 0.)], dim=1)
         q = self.scale * self.query(x[:, g:]).reshape(B, N - g, H, M).transpose(1, 2)
         kv = self.kv(x).reshape(B, N, 2, H, M).permute(2, 0, 3, 1, 4)
         k, v = kv[0], kv[1]
         a1 = self.attn_drop((q @ k[:, :, :g].transpose(-2, -1)).softmax(dim=-1))
-        x1 = self.proj((a1 @ v[:, :, :g]).transpose(1, 2).reshape(B, N - g, C))
+        o1 = (a1 @ v[:, :, :g]).transpose(1, 2).reshape(B, N - g, C)
+        if keep is not None:
+            o1 = torch.where(keep[:, :, None], o1, 0.)
+        x1 = self.proj(o1)
         qg = self.scale * self.query_global(x[:, :g]).reshape(B, g, H, M).transpose(1, 2)
         kvg = self.kv_global(x).reshape(B, N, 2, H, M).permute(2, 0, 3, 1, 4)
-        a0 = qg @ kvg[0].transpose(-2, -1)
+        kg, vg = kvg[0], kvg[1]
+        a0 = qg @ kg.transpose(-2, -1)
         if self.rpe:
             a0 = a0 + torch.cat([self.g2g_relative_position_bias,
                                  self.g2l_relative_position_bias[0].unsqueeze(-1).expand(-1, -1, N - g)], dim=-1)
-        x0 = self.proj_global((self.attn_drop(a0.softmax(dim=-1)) @ kvg[1]).transpose(1, 2).reshape(B, g, C))
+        if keep is not None:
+            a0 = a0.masked_fill(~torch.cat([keep.new_ones(B, g), keep], dim=1)[:, None, None, :], float("-inf"))
+        x0 = self.proj_global((self.attn_drop(a0.softmax(dim=-1)) @ vg).transpose(1, 2).reshape(B, g, C))
         return self.proj_drop(torch.cat((x0, x1), dim=1))
 
     @staticmethod

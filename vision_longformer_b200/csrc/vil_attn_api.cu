@@ -151,7 +151,8 @@ int check_common(const VilAttnParams* p, const vil::Geo& g, bool bwd) {
   return VIL_OK;
 }
 
-int run(const VilAttnParams* p, void* stream, bool bwd) {
+// image_hw: the per-image grids of a sized call (device memory), NULL for the unsized entry points
+int run(const VilAttnParams* p, void* stream, bool bwd, const int32_t* image_hw) {
   vil::Geo g;
   int rc = make_geo(p, &g);
   if (rc) return rc;
@@ -160,15 +161,19 @@ int run(const VilAttnParams* p, void* stream, bool bwd) {
   const int tc_ok = vil::tc_supported(p, g, bwd);
   int impl = p->impl;
   if (impl == VIL_IMPL_AUTO) impl = tc_ok ? VIL_IMPL_WGMMA : VIL_IMPL_SIMT;
+  const char* name;
   if (impl == VIL_IMPL_WGMMA) {
     if (!tc_ok) return fail(VIL_E_UNSUPPORTED, "the wgmma family does not cover this configuration: %s", vil::tc_why_not(p, g, bwd));
-    rc = bwd ? vil::tc_backward(p, g, s) : vil::tc_forward(p, g, s);
-    if (rc == VIL_OK) g_last_impl = "wgmma";
-    return rc;
+    rc = bwd ? vil::tc_backward(p, g, s, image_hw) : vil::tc_forward(p, g, s, image_hw);
+    name = "wgmma";
+  } else {
+    if (impl != VIL_IMPL_SIMT) return fail(VIL_E_BADARG, "impl must be VIL_IMPL_AUTO, _SIMT or _TCGEN05");
+    rc = vil::simt_run(p, g, s, bwd, image_hw);
+    name = "simt";
   }
-  if (impl != VIL_IMPL_SIMT) return fail(VIL_E_BADARG, "impl must be VIL_IMPL_AUTO, _SIMT or _TCGEN05");
-  rc = vil::simt_run(p, g, s, bwd);
-  if (rc == VIL_OK) g_last_impl = "simt";
+  // the rows of off-image tokens, which the kernels above leave alone, get their zeros (and lse its -inf)
+  if (rc == VIL_OK && image_hw != nullptr) rc = vil::simt_zero_off_image(p, g, s, bwd, image_hw);
+  if (rc == VIL_OK) g_last_impl = name;
   return rc;
 }
 
@@ -300,7 +305,16 @@ int vil_attn_wgmma_supported(const VilAttnParams* p) {
   return vil::tc_supported(p, g, false) ? 1 : 0;
 }
 
-int vil_attn_fwd_sm100(const VilAttnParams* p, void* stream) { return run(p, stream, false); }
-int vil_attn_bwd_sm100(const VilAttnParams* p, void* stream) { return run(p, stream, true); }
+int vil_attn_fwd_sm100(const VilAttnParams* p, void* stream) { return run(p, stream, false, nullptr); }
+int vil_attn_bwd_sm100(const VilAttnParams* p, void* stream) { return run(p, stream, true, nullptr); }
+
+int vil_attn_fwd_sized_sm100(const VilAttnParams* p, const int32_t* image_hw, void* stream) {
+  if (image_hw == nullptr) return fail(VIL_E_BADARG, "image_hw is NULL (the sized entry points need the per-image grids)");
+  return run(p, stream, false, image_hw);
+}
+int vil_attn_bwd_sized_sm100(const VilAttnParams* p, const int32_t* image_hw, void* stream) {
+  if (image_hw == nullptr) return fail(VIL_E_BADARG, "image_hw is NULL (the sized entry points need the per-image grids)");
+  return run(p, stream, true, image_hw);
+}
 
 }  // extern "C"

@@ -35,16 +35,42 @@ struct Geo {
   int d;
 };
 
+// Per-image grids (vil_attn_fwd_sized_sm100 / _bwd_sized_sm100): image b's grid of ih x iw tokens, its image_hw entry
+// clamped to [1, nx] x [1, ny] so that a bad entry cannot address past the padded grid; without sizes (image_hw == NULL)
+// the whole nx x ny grid.
+__device__ __forceinline__ void image_extent(const Geo& g, const int* __restrict__ image_hw, int b, int& ih, int& iw) {
+  ih = g.nx; iw = g.ny;
+  if (image_hw != nullptr) {
+    ih = min(max(image_hw[2 * b], 1), g.nx);
+    iw = min(max(image_hw[2 * b + 1], 1), g.ny);
+  }
+}
+// local token t (row t / ny, column t % ny of the padded grid) lies on an ih x iw image
+__device__ __forceinline__ bool on_image(const Geo& g, int ih, int iw, long long t) { return t / g.ny < ih && t % g.ny < iw; }
+
 // Dilated calls (d > 1) run the operator on each of the d^2 residue sub-grids of the image: residue (a, b) holds the local
 // tokens (a + d r, b + d c).  mx / my then count the chunks of a virtual grid of d mx0 x d my0 chunks (mx0 x my0: the chunk
 // grid of the largest sub-grid, residue (0, 0)); virtual chunk (R', C') is chunk (R' / d, C' / d) of residue
 // (R' % d, C' % d).  Every grid, CTA count and workspace size derived from mx / my thereby covers the d^2 sub-grids, and a
 // CTA whose chunk lies outside its (smaller) sub-grid exits.  SubGrid is the geometry a CTA's masks use: its sub-grid's
 // tokens, padding and chunk counts, and its residue; undilated, Geo's own.
+// The same instantiations (DIL) run calls with per-image grids, dilated or not (d = 1): the sub-grids are then those of
+// image b's ih x iw crop (image_extent), while token addresses keep the padded grid's row stride geo.ny (VIL_SUB_*).
 template <bool DIL> struct SubGrid;
 template <> struct SubGrid<true> {
   int nx_, ny_, padx_, pady_, mx_, my_;
   int r0_, c0_;         // residue (a, b)
+  // the residue's sub-grid of image b (image_extent); r0_, c0_ set
+  __device__ __forceinline__ void fit(const Geo& g, const int* __restrict__ image_hw, int b) {
+    int ih, iw;
+    image_extent(g, image_hw, b, ih, iw);
+    nx_ = (ih - r0_ + g.d - 1) / g.d;
+    ny_ = (iw - c0_ + g.d - 1) / g.d;
+    padx_ = (g.w - nx_ % g.w) % g.w;
+    pady_ = (g.w - ny_ % g.w) % g.w;
+    mx_ = (nx_ + padx_) / g.w;
+    my_ = (ny_ + pady_) / g.w;
+  }
   __device__ __forceinline__ int nx() const { return nx_; }
   __device__ __forceinline__ int ny() const { return ny_; }
   __device__ __forceinline__ int padx() const { return padx_; }
@@ -68,19 +94,14 @@ template <> struct SubGrid<false> {
   __device__ __forceinline__ int c0() const { return 0; }
 };
 
-// The CTA's sub-grid; R, C: in the virtual chunk position, out the chunk position in the sub-grid
+// The CTA's sub-grid in image b; R, C: in the virtual chunk position, out the chunk position in the sub-grid
 template <bool DIL>
-__device__ __forceinline__ SubGrid<DIL> sub_grid(const Geo& g, int& R, int& C) {
+__device__ __forceinline__ SubGrid<DIL> sub_grid(const Geo& g, int& R, int& C, const int* __restrict__ image_hw, int b) {
   if constexpr (DIL) {
     SubGrid<true> s;
     s.r0_ = R % g.d; R /= g.d;
     s.c0_ = C % g.d; C /= g.d;
-    s.nx_ = (g.nx - s.r0_ + g.d - 1) / g.d;
-    s.ny_ = (g.ny - s.c0_ + g.d - 1) / g.d;
-    s.padx_ = (g.w - s.nx_ % g.w) % g.w;
-    s.pady_ = (g.w - s.ny_ % g.w) % g.w;
-    s.mx_ = (s.nx_ + s.padx_) / g.w;
-    s.my_ = (s.ny_ + s.pady_) / g.w;
+    s.fit(g, image_hw, b);
     return s;
   } else {
     return SubGrid<false>{g};
@@ -91,7 +112,7 @@ __device__ __forceinline__ SubGrid<DIL> sub_grid(const Geo& g, int& R, int& C) {
 // (read through SubGrid<false>, the same values compile to differently scheduled code).
 #define VIL_SG(f) (DIL ? sg.f() : geo.f)
 
-// a CTA of a dilated call whose chunk lies outside its sub-grid (never one of an undilated call)
+// a CTA of a dilated or sized call whose chunk lies outside its sub-grid (never one of the plain instantiations)
 template <bool DIL>
 __device__ __forceinline__ bool off_sub_grid(const SubGrid<DIL>& s, int R, int C) {
   if constexpr (DIL) return R >= s.mx() || C >= s.my();

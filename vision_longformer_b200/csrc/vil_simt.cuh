@@ -61,7 +61,7 @@ __device__ __forceinline__ ChunkId decode_block(const Geo& g, int bid) {
 template <typename T, int HD, int L, bool DROP, bool DIL = false>
 __global__ void __launch_bounds__(64 * L, L == 4 ? 1 : 0)
 simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
-               const float* __restrict__ table, const float* __restrict__ g2l) {
+               const float* __restrict__ table, const float* __restrict__ g2l, const int* __restrict__ image_hw) {
   using TL = Tile<HD, L>;
   constexpr int HP = TL::HP, HS = TL::HS;
   extern __shared__ float smem[];
@@ -81,7 +81,7 @@ simt_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse,
   const int w = geo.w, D = geo.D;
 
   for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
-  const auto sg = sub_grid<DIL>(geo, R, C);
+  const auto sg = sub_grid<DIL>(geo, R, C, image_hw, b);
   if (off_sub_grid<DIL>(sg, R, C)) return;
 
   const int l = cid.piece * 64 + slot;
@@ -221,11 +221,13 @@ __device__ __forceinline__ float dot8(const float (&a)[8], const float (&b)[8]) 
 // ----------------------------------------------------------------------------------------------
 // forward, global query rows: dense attention of the nglo global queries over all N keys
 // (longformer2d.py:210-227).  CTA = one (b, h, a); 8 warps x (32/LPR) rows per iteration.
+// SIZED (per-image grids): only the global keys and the keys on image b's grid take part; the others are never loaded
+// (a masked score alone would still let a NaN through 0 * v).
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO = T, bool DROP = false>   // TO: element type of the OUTPUT (fp32 in the parity build)
+template <typename T, int HD, typename TO = T, bool DROP = false, bool SIZED = false>   // TO: element type of the OUTPUT
 __global__ void __launch_bounds__(256)
 simt_fwd_global(Geo geo, T4 qg, T4 kg, T4 vg, T4 og, float* __restrict__ lse_g, const float* __restrict__ g2l,
-                const float* __restrict__ g2g) {
+                const float* __restrict__ g2g, const int* __restrict__ image_hw) {
   constexpr int LPR = HD / 8, RPW = 32 / LPR, ROWS = 8 * RPW;
   __shared__ float red_m[8], red_l[8];
   __shared__ float red_o[8][HD];
@@ -240,13 +242,21 @@ simt_fwd_global(Geo geo, T4 qg, T4 kg, T4 vg, T4 og, float* __restrict__ lse_g, 
 #pragma unroll
   for (int i = 0; i < 8; ++i) oacc[i] = 0.f;
   const float bl = geo.has_bias ? g2l[(long long)h * geo.g + a] : 0.f;       // g2l[0][h][a]
+  int ih = 0, iw = 0;
+  if constexpr (SIZED) image_extent(geo, image_hw, b, ih, iw);
   for (int base = row0 + warp * RPW; base < row1; base += ROWS) {
     const int j = base + rw;
-    const bool valid = j < row1;
+    bool valid = j < row1;
     const int jc = valid ? j : row1 - 1;
     float kk[8], vv[8];
-    load_seg<T, 8>(row_ptr<T>(kg, b, h, jc), 8 * sub, D, kk);
-    load_seg<T, 8>(row_ptr<T>(vg, b, h, jc), 8 * sub, D, vv);
+    if (SIZED && !(jc < geo.g || on_image(geo, ih, iw, jc - geo.g))) {
+      valid = false;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
+    } else {
+      load_seg<T, 8>(row_ptr<T>(kg, b, h, jc), 8 * sub, D, kk);
+      load_seg<T, 8>(row_ptr<T>(vg, b, h, jc), 8 * sub, D, vv);
+    }
     const float sp = group_sum<LPR>(dot8(q8, kk));
     float bias = bl;
     if (geo.has_bias && jc < geo.g) bias = g2g[((long long)h * geo.g + a) * geo.g + jc];
@@ -336,7 +346,7 @@ template <typename T, int HD, int L, bool DROP, bool TAB, bool DIL = false>
 __global__ void __launch_bounds__(64 * L, L == 4 ? 1 : (TAB && HD <= 8 ? 4 : 0))
 simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse,
             const float* __restrict__ delta, const float* __restrict__ table,
-            const float* __restrict__ g2l, float* __restrict__ tpart) {
+            const float* __restrict__ g2l, float* __restrict__ tpart, const int* __restrict__ image_hw) {
   using TL = Tile<HD, L>;
   constexpr int HP = TL::HP, HS = TL::HS;
   extern __shared__ float smem[];
@@ -363,18 +373,26 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
     acc = tpart + (long long)blockIdx.x * tabn;
     for (int i = tid; i < tabn; i += 64 * L) acc[i] = 0.f;
   }
-  const auto sg = sub_grid<DIL>(geo, R, C);
-  if (off_sub_grid<DIL>(sg, R, C)) return;             // after zeroing its row of table partials
+  auto sg = sub_grid<DIL>(geo, R, C, image_hw, cid.b);
+  // after zeroing its row of table partials; TAB: per image below, since the sub-grid depends on the image's size
+  if (!TAB && off_sub_grid<DIL>(sg, R, C)) return;
 
   const int l = cid.piece * 64 + slot;
   const int qr = l / w, qc = l % w;
   const int r = R * w + qr, c = C * w + qc;
-  const bool qvalid = (l < geo.w2) && (r < VIL_SG(nx)) && (c < VIL_SG(ny));
+  bool qvalid = (l < geo.w2) && (r < VIL_SG(nx)) && (c < VIL_SG(ny));
   const long long tokq = VIL_SUB_TOK(r, c);
 
   const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
   for (int it = 0; it < nimg; ++it) {
   const int b = cid.b + it * geo.nslice;
+  if constexpr (TAB && DIL) {          // CTA-uniform: skip an image the chunk lies outside of; the query row's validity
+    if (it > 0 && image_hw != nullptr) {   // (hoisted above for one image per CTA) follows the image's sub-grid
+      sg.fit(geo, image_hw, b);
+      qvalid = (l < geo.w2) && (r < sg.nx()) && (c < sg.ny());
+    }
+    if (off_sub_grid<DIL>(sg, R, C)) continue;
+  }
   float qh[HP], doh[HP], dqh[HP];
 #pragma unroll
   for (int i = 0; i < HP; ++i) { qh[i] = 0.f; doh[i] = 0.f; dqh[i] = 0.f; }
@@ -495,7 +513,7 @@ simt_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ 
 template <typename T, int HD, int L, bool DROP, bool DIL = false>
 __global__ void __launch_bounds__(64 * L, L == 4 ? 1 : 0)
 simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
-             const float* __restrict__ delta, const float* __restrict__ table) {
+             const float* __restrict__ delta, const float* __restrict__ table, const int* __restrict__ image_hw) {
   using TL = Tile<HD, L>;
   constexpr int HP = TL::HP, HS = TL::HS;
   extern __shared__ float smem[];
@@ -517,7 +535,7 @@ simt_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __res
   const int tid = threadIdx.x, slot = tid >> (L / 2), part = tid & (L - 1);
   const int w = geo.w, D = geo.D;
   for (int i = tid; i < tabn; i += 64 * L) tab[i] = table[(long long)i * geo.H + h];
-  const auto sg = sub_grid<DIL>(geo, KR, KC);
+  const auto sg = sub_grid<DIL>(geo, KR, KC, image_hw, b);
   if (off_sub_grid<DIL>(sg, KR, KC)) return;
 
   const int lk = cid.piece * 64 + slot;
@@ -627,12 +645,14 @@ __device__ __forceinline__ float block_sum_256(float v, float* red /*[8]*/) {
 // ----------------------------------------------------------------------------------------------
 // backward, global KEY columns seen by the local queries: dk[t], dv[t] for t < nglo and, with the bias table, this
 // image's term of d_g2l[1][h][t] into pcol[b][h][t] (summed over the images by simt_bwd_bias_reduce).
-// CTA = one (b, h, t); row groups stride over the local queries.
+// CTA = one (b, h, t); row groups stride over the local queries.  SIZED (per-image grids): only the queries on image b's
+// grid; the others, whose d_o, lse and delta are arbitrary, are never loaded.
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO = T, bool DROP = false>
+template <typename T, int HD, typename TO = T, bool DROP = false, bool SIZED = false>
 __global__ void __launch_bounds__(256)
 simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse,
-              const float* __restrict__ delta, const float* __restrict__ g2l, float* __restrict__ pcol) {
+              const float* __restrict__ delta, const float* __restrict__ g2l, float* __restrict__ pcol,
+              const int* __restrict__ image_hw) {
   constexpr int LPR = HD / 8, RPW = 32 / LPR, ROWS = 8 * RPW;
   __shared__ float red[8];
   __shared__ float accs[8][2][HD];
@@ -649,14 +669,22 @@ simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
 #pragma unroll
   for (int i = 0; i < 8; ++i) { adk[i] = 0.f; adv[i] = 0.f; }
   const long long base_l = ((long long)b * geo.H + h) * geo.Nloc;
+  int ih = 0, iw = 0;
+  if constexpr (SIZED) image_extent(geo, image_hw, b, ih, iw);
   for (int base = row0 + warp * RPW; base < row1; base += ROWS) {
     const int i2 = base + rw;
-    const bool valid = i2 < row1;
+    bool valid = i2 < row1;
     const int ic = valid ? i2 : row1 - 1;
-    float qq[8], gg[8];
-    load_seg<T, 8>(row_ptr<T>(q, b, h, ic), 8 * sub, D, qq);
-    load_seg<T, 8>(row_ptr<T>(d_o, b, h, ic), 8 * sub, D, gg);
-    const float ls = lse[base_l + ic], dl = delta[base_l + ic];
+    float qq[8], gg[8], ls, dl;
+    if (SIZED && !on_image(geo, ih, iw, ic)) {
+      valid = false; ls = 0.f; dl = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { qq[i] = 0.f; gg[i] = 0.f; }
+    } else {
+      load_seg<T, 8>(row_ptr<T>(q, b, h, ic), 8 * sub, D, qq);
+      load_seg<T, 8>(row_ptr<T>(d_o, b, h, ic), 8 * sub, D, gg);
+      ls = lse[base_l + ic]; dl = delta[base_l + ic];
+    }
     const float sp = group_sum<LPR>(dot8(qq, k8)), dpp = group_sum<LPR>(dot8(gg, v8));
     float p = valid ? __expf(fmaf(geo.scale, sp, bias) - ls) : 0.f;
     float dpk = dpp;
@@ -696,13 +724,15 @@ simt_bwd_gcol(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __re
 // terms of d_g2g into pgg[b][h][a][j] and of d_g2l[0] into prow[b][h][a] (summed over the images by simt_bwd_bias_reduce).
 // CTA = one (b, h); row groups stride over the keys.  `accumulate` != 0: add into dkg/dvg (they alias dk/dv,
 // already written by the dK/dV pass and simt_bwd_gcol earlier on the same stream); else overwrite.
+// SIZED (per-image grids): as simt_fwd_global, the keys off image b's grid are never loaded and get P = 0.
 // ----------------------------------------------------------------------------------------------
-template <typename T, int HD, typename TO = T, bool DROP = false>
-__global__ void __launch_bounds__(256)
+template <typename T, int HD, typename TO = T, bool DROP = false, bool SIZED = false>
+__global__ void __launch_bounds__(256, SIZED ? 2 : 0)   // SIZED: at ptxas's own choice of 80 registers it spills
 simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
               const float* __restrict__ lse_g, const float* __restrict__ delta_g,
               const float* __restrict__ g2l, const float* __restrict__ g2g,
-              float* __restrict__ prow, float* __restrict__ pgg, int accumulate, int rmw_rows) {
+              float* __restrict__ prow, float* __restrict__ pgg, int accumulate, int rmw_rows,
+              const int* __restrict__ image_hw) {
   // rmw_rows: keys [0, rmw_rows) get their dkg / dvg rows updated here
   constexpr int LPR = HD / 8, RPW = 32 / LPR, ROWS = 8 * RPW;
   __shared__ float red[8];
@@ -711,6 +741,8 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
   const int b = blockIdx.x / geo.H;
   const int tid = threadIdx.x, D = geo.D, lane = tid & 31, warp = tid >> 5, sub = lane % LPR, rw = lane / LPR;
   const int row0 = 0, row1 = geo.N;
+  int ih = 0, iw = 0;
+  if constexpr (SIZED) image_extent(geo, image_hw, b, ih, iw);
   for (int a = 0; a < geo.g; ++a) {
     float q8[8], g8[8];
     load_seg<T, 8>(row_ptr<T>(qg, b, h, a), 8 * sub, D, q8);
@@ -727,8 +759,14 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
       const bool valid = j < row1;
       const int jc = valid ? j : row1 - 1;
       float kk[8], vv[8], ok_[8], ov_[8];
-      load_seg<T, 8>(row_ptr<T>(kg, b, h, jc), 8 * sub, D, kk);
-      load_seg<T, 8>(row_ptr<T>(vg, b, h, jc), 8 * sub, D, vv);
+      const bool live = !SIZED || jc < geo.g || on_image(geo, ih, iw, jc - geo.g);
+      if (SIZED && !live) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { kk[i] = 0.f; vv[i] = 0.f; }
+      } else {
+        load_seg<T, 8>(row_ptr<T>(kg, b, h, jc), 8 * sub, D, kk);
+        load_seg<T, 8>(row_ptr<T>(vg, b, h, jc), 8 * sub, D, vv);
+      }
       const bool rmw = base < rmw_rows;                 // warp-uniform up to the last partial row batch
       if (add && rmw) {
         load_seg<TO, 8>(row_ptr<TO>(dkg, b, h, jc), 8 * sub, D, ok_);
@@ -740,7 +778,7 @@ simt_bwd_grow(Geo geo, T4 qg, T4 kg, T4 vg, T4 d_og, T4 dqg, T4 dkg, T4 dvg,
       const float sp = group_sum<LPR>(dot8(q8, kk)), dpp = group_sum<LPR>(dot8(g8, vv));
       float bias = bl;
       if (geo.has_bias && jc < geo.g) bias = g2g[((long long)h * geo.g + a) * geo.g + jc];
-      const float p = valid ? __expf(fmaf(geo.scale, sp, bias) - lg) : 0.f;
+      const float p = valid && live ? __expf(fmaf(geo.scale, sp, bias) - lg) : 0.f;
       float km = 1.f;                              // dropout: dS = P (dP keep / (1 - p) - delta), dV += P keep / (1 - p) dO
       if constexpr (DROP) km = drop_keep(geo, (uint32_t)a, (uint32_t)jc, 2u * (uint32_t)(b * geo.H + h) + 1u) ? geo.drop_scale : 0.f;
       const float ds = DROP ? p * (dpp * km - dg) : p * (dpp - dg);
@@ -817,32 +855,62 @@ simt_bwd_bias_reduce(Geo geo, const float* __restrict__ tpart, const float* __re
   }
 }
 
+// ----------------------------------------------------------------------------------------------
+// Sized calls (per-image grids): exact zeros in the rows of the local tokens off image b's grid, which no other kernel
+// writes -- row t + off[i] of each of the n outputs rows[i] -- and lse = -inf there (an empty softmax) when lse is
+// given.  One warp per local row; E: an unsigned integer of the element's size (zero bits are 0 in fp32, bf16 and fp16).
+// ----------------------------------------------------------------------------------------------
+struct OffImageRows {
+  T4 rows[5];
+  int off[5];
+  int n;
+  float* lse;
+};
+template <typename E>
+__global__ void __launch_bounds__(256)
+simt_zero_off_image(Geo geo, OffImageRows z, const int* __restrict__ image_hw) {
+  const long long nrows = (long long)geo.B * geo.H * geo.Nloc;
+  const long long stride = (long long)gridDim.x * (blockDim.x >> 5);
+  const int lane = threadIdx.x & 31;
+  for (long long x = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); x < nrows; x += stride) {
+    const long long t = x % geo.Nloc, bh = x / geo.Nloc;
+    const int b = (int)(bh / geo.H), h = (int)(bh % geo.H);
+    int ih, iw;
+    image_extent(geo, image_hw, b, ih, iw);
+    if (on_image(geo, ih, iw, t)) continue;                  // warp-uniform
+    for (int i = 0; i < z.n; ++i)
+      for (int c = lane; c < geo.D; c += 32) row_ptr_w<E>(z.rows[i], b, h, t + z.off[i])[c] = E(0);
+    if (z.lse != nullptr && lane == 0) z.lse[x] = -INFINITY;
+  }
+}
+
 // ---------------------------------------------------------------- host launchers (both kernel families)
+// image_hw != NULL (a sized call) runs the SIZED instantiations
 template <typename T, int HD, typename TO = T>
 inline void launch_global_fwd_kernels(const Geo& g, T4 qg, T4 kg, T4 vg, T4 og, float* lse_g, const float* g2l,
-                                      const float* g2g, cudaStream_t s) {
-  if (g.drop_p > 0.f) simt_fwd_global<T, HD, TO, true><<<g.B * g.H * g.g, 256, 0, s>>>(g, qg, kg, vg, og, lse_g, g2l, g2g);
-  else simt_fwd_global<T, HD, TO><<<g.B * g.H * g.g, 256, 0, s>>>(g, qg, kg, vg, og, lse_g, g2l, g2g);
+                                      const float* g2g, const int* image_hw, cudaStream_t s) {
+  const auto kernel = g.drop_p > 0.f ? (image_hw ? simt_fwd_global<T, HD, TO, true, true> : simt_fwd_global<T, HD, TO, true>)
+                                     : (image_hw ? simt_fwd_global<T, HD, TO, false, true> : simt_fwd_global<T, HD, TO>);
+  kernel<<<g.B * g.H * g.g, 256, 0, s>>>(g, qg, kg, vg, og, lse_g, g2l, g2g, image_hw);
 }
 template <typename T, int HD, typename TO = T>
 inline void launch_global_bwd_kernels(const Geo& g, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, T4 qg, T4 kg, T4 vg, T4 d_og,
                                       T4 dqg, T4 dkg, T4 dvg, const float* lse, const float* delta, const float* lse_g,
                                       const float* delta_g, const float* g2l, const float* g2g, float* gpart,
-                                      int accumulate, int rmw_rows, cudaStream_t s) {
+                                      int accumulate, int rmw_rows, const int* image_hw, cudaStream_t s) {
   // gpart: the global-bias partials (vil_common.cuh, ws_off_glob), read only with the bias table
   const long long bhg = (long long)g.B * g.H * g.g;
   float* pcol = gpart;
   float* prow = gpart ? gpart + bhg : nullptr;
   float* pgg = gpart ? gpart + 2 * bhg : nullptr;
-  if (g.drop_p > 0.f) {
-    simt_bwd_gcol<T, HD, TO, true><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, pcol);
-    simt_bwd_grow<T, HD, TO, true><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, prow,
-                                                             pgg, accumulate, rmw_rows);
-    return;
-  }
-  simt_bwd_gcol<T, HD, TO><<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, pcol);
-  simt_bwd_grow<T, HD, TO><<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, prow, pgg,
-                                                  accumulate, rmw_rows);
+  const bool drop = g.drop_p > 0.f;
+  const auto gcol = drop ? (image_hw ? simt_bwd_gcol<T, HD, TO, true, true> : simt_bwd_gcol<T, HD, TO, true>)
+                         : (image_hw ? simt_bwd_gcol<T, HD, TO, false, true> : simt_bwd_gcol<T, HD, TO>);
+  const auto grow = drop ? (image_hw ? simt_bwd_grow<T, HD, TO, true, true> : simt_bwd_grow<T, HD, TO, true>)
+                         : (image_hw ? simt_bwd_grow<T, HD, TO, false, true> : simt_bwd_grow<T, HD, TO>);
+  gcol<<<g.B * g.H * g.g, 256, 0, s>>>(g, q, k, v, d_o, dk, dv, lse, delta, g2l, pcol, image_hw);
+  grow<<<g.B * g.H, 256, 0, s>>>(g, qg, kg, vg, d_og, dqg, dkg, dvg, lse_g, delta_g, g2l, g2g, prow, pgg, accumulate, rmw_rows,
+                                 image_hw);
 }
 
 }  // namespace vil

@@ -63,85 +63,91 @@ const char* why_not(const VilAttnParams* p, const Geo& g, bool bwd) {
 
 long long blocks(const Geo& g) { return (long long)g.B * g.H * g.mx * g.my * g.npc; }
 
+// a dilated (g.d > 1) or sized call runs the DIL instantiations over the residue sub-grids of each image
+// (vil_common.cuh, SubGrid)
+inline bool sub_grids(const Geo& g, const int* image_hw) { return g.d > 1 || image_hw != nullptr; }
+
 template <typename T, int HD, typename TO, bool DROP>
-int forward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+int forward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s, const int* image_hw) {
   int rc;
   if (!(p->skip_mask & 2)) {
     const size_t sm = wg::FwdSmem<T, HD>::total(table_floats(g));
-    // a dilated call (g.d > 1) runs the DIL instantiation over the d^2 residue sub-grids (vil_common.cuh, SubGrid)
-    const auto kernel = g.d > 1 ? wg::wg_fwd_local<T, HD, TO, DROP, true> : wg::wg_fwd_local<T, HD, TO, DROP>;
+    const auto kernel = sub_grids(g, image_hw) ? wg::wg_fwd_local<T, HD, TO, DROP, true> : wg::wg_fwd_local<T, HD, TO, DROP>;
     if ((rc = set_smem(kernel, sm))) return rc;
-    kernel<<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse, p->bias_table, p->g2l);
+    kernel<<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->o), p->lse, p->bias_table, p->g2l,
+                                                         image_hw);
     count_launch();
     if ((rc = launch_check("wgmma_fwd_local"))) return rc;
   }
-  if (g.g > 0 && !(p->skip_mask & 1)) return simt_global_fwd(p, g, s);
+  if (g.g > 0 && !(p->skip_mask & 1)) return simt_global_fwd(p, g, s, image_hw);
   return VIL_OK;
 }
 
 // backward pass 1; TAB (the bias table): nslice image slices per (head, chunk, piece), table partials into the workspace
 template <typename T, int HD, typename TO, bool DROP, bool TAB>
-int dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+int dq_pass(const VilAttnParams* p, const Geo& g, cudaStream_t s, const int* image_hw) {
   int rc;
   const size_t sm = wg::DqSmem<T, HD>::total(table_floats(g), TAB);
-  const auto kernel = g.d > 1 ? wg::wg_bwd_dq<T, HD, TO, DROP, TAB, true> : wg::wg_bwd_dq<T, HD, TO, DROP, TAB>;
+  const auto kernel = sub_grids(g, image_hw) ? wg::wg_bwd_dq<T, HD, TO, DROP, TAB, true> : wg::wg_bwd_dq<T, HD, TO, DROP, TAB>;
   if ((rc = set_smem(kernel, sm))) return rc;
   const long long ctas = TAB ? tab_ctas(g) : blocks(g);
   kernel<<<(unsigned)ctas, wg::kThreads, sm, s>>>(
       g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dq), p->lse, ws_at(p, 0), p->bias_table, p->g2l,
-      TAB ? ws_at(p, ws_off_tab(g)) : nullptr);
+      TAB ? ws_at(p, ws_off_tab(g)) : nullptr, image_hw);
   count_launch();
   return launch_check("wgmma_bwd_dq");
 }
 
 template <typename T, int HD, typename TO, bool DROP>
-int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s) {
+int backward_t(const VilAttnParams* p, const Geo& g, cudaStream_t s, const int* image_hw) {
   int rc;
   if (!(p->skip_mask & 8) && (rc = simt_delta(p, g, s))) return rc;
   float* delta = static_cast<float*>(p->workspace);
   const int tabn = table_floats(g);
   if (!(p->skip_mask & 2)) {
-    if ((rc = g.has_bias ? dq_pass<T, HD, TO, DROP, true>(p, g, s) : dq_pass<T, HD, TO, DROP, false>(p, g, s))) return rc;
+    if ((rc = g.has_bias ? dq_pass<T, HD, TO, DROP, true>(p, g, s, image_hw) : dq_pass<T, HD, TO, DROP, false>(p, g, s, image_hw)))
+      return rc;
   }
   if (!(p->skip_mask & 4)) {
     const size_t sm = wg::DkvSmem<T, HD>::total(tabn, DROP);
-    const auto kernel = g.d > 1 ? wg::wg_bwd_dkv<T, HD, TO, DROP, true> : wg::wg_bwd_dkv<T, HD, TO, DROP>;
+    const auto kernel = sub_grids(g, image_hw) ? wg::wg_bwd_dkv<T, HD, TO, DROP, true> : wg::wg_bwd_dkv<T, HD, TO, DROP>;
     if ((rc = set_smem(kernel, sm))) return rc;
     kernel<<<(unsigned)blocks(g), wg::kThreads, sm, s>>>(g, t4(p->q), t4(p->k), t4(p->v), t4(p->d_o), t4(p->dk), t4(p->dv), p->lse,
-                                                         delta, p->bias_table);
+                                                         delta, p->bias_table, image_hw);
     count_launch();
     if ((rc = launch_check("wgmma_bwd_dkv"))) return rc;
   }
-  if (g.g > 0 && !(p->skip_mask & 1) && (rc = simt_global_bwd(p, g, s, g.N))) return rc;
+  if (g.g > 0 && !(p->skip_mask & 1) && (rc = simt_global_bwd(p, g, s, g.N, image_hw))) return rc;
   return simt_bias_reduce(p, g, s);
 }
 
 template <typename T, typename TO, bool DROP>
-int dispatch_hd_drop(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
+int dispatch_hd_drop(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd, const int* hw) {
   switch (head_tile(g.D)) {
-    case 16: return bwd ? backward_t<T, 16, TO, DROP>(p, g, s) : forward_t<T, 16, TO, DROP>(p, g, s);
-    case 32: return bwd ? backward_t<T, 32, TO, DROP>(p, g, s) : forward_t<T, 32, TO, DROP>(p, g, s);
-    case 64: return bwd ? backward_t<T, 64, TO, DROP>(p, g, s) : forward_t<T, 64, TO, DROP>(p, g, s);
+    case 16: return bwd ? backward_t<T, 16, TO, DROP>(p, g, s, hw) : forward_t<T, 16, TO, DROP>(p, g, s, hw);
+    case 32: return bwd ? backward_t<T, 32, TO, DROP>(p, g, s, hw) : forward_t<T, 32, TO, DROP>(p, g, s, hw);
+    case 64: return bwd ? backward_t<T, 64, TO, DROP>(p, g, s, hw) : forward_t<T, 64, TO, DROP>(p, g, s, hw);
     default:
       if constexpr (wg::kSplit<T>) return shared_fail(VIL_E_UNSUPPORTED, "split fp32 kernels stop at head dim 64");
-      else return bwd ? backward_t<T, 128, TO, DROP>(p, g, s) : forward_t<T, 128, TO, DROP>(p, g, s);
+      else return bwd ? backward_t<T, 128, TO, DROP>(p, g, s, hw) : forward_t<T, 128, TO, DROP>(p, g, s, hw);
   }
 }
 
 template <typename T, typename TO>
-int dispatch_hd(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
-  return g.drop_p > 0.f ? dispatch_hd_drop<T, TO, true>(p, g, s, bwd) : dispatch_hd_drop<T, TO, false>(p, g, s, bwd);
+int dispatch_hd(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd, const int* hw) {
+  return g.drop_p > 0.f ? dispatch_hd_drop<T, TO, true>(p, g, s, bwd, hw) : dispatch_hd_drop<T, TO, false>(p, g, s, bwd, hw);
 }
 
-int run(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd) {
+int run(const VilAttnParams* p, const Geo& g, cudaStream_t s, bool bwd, const int* hw) {
   if (p->dtype == VIL_F32) {   // why_not admits fp32 only with VIL_FLAG_F32_SPLIT
     note_kernel(bwd ? "wgmma_f32split_bwd" : "wgmma_f32split_fwd");
-    return dispatch_hd<float, float>(p, g, s, bwd);
+    return dispatch_hd<float, float>(p, g, s, bwd, hw);
   }
   note_kernel(bwd ? "wgmma_bwd" : "wgmma_fwd");
   if (p->dtype == VIL_BF16)
-    return out_f32(p) ? dispatch_hd<__nv_bfloat16, float>(p, g, s, bwd) : dispatch_hd<__nv_bfloat16, __nv_bfloat16>(p, g, s, bwd);
-  return out_f32(p) ? dispatch_hd<__half, float>(p, g, s, bwd) : dispatch_hd<__half, __half>(p, g, s, bwd);
+    return out_f32(p) ? dispatch_hd<__nv_bfloat16, float>(p, g, s, bwd, hw)
+                      : dispatch_hd<__nv_bfloat16, __nv_bfloat16>(p, g, s, bwd, hw);
+  return out_f32(p) ? dispatch_hd<__half, float>(p, g, s, bwd, hw) : dispatch_hd<__half, __half>(p, g, s, bwd, hw);
 }
 
 }  // namespace
@@ -151,7 +157,7 @@ const char* tc_why_not(const VilAttnParams* p, const Geo& g, bool bwd) {
   return w ? w : "supported";
 }
 int tc_supported(const VilAttnParams* p, const Geo& g, bool bwd) { return why_not(p, g, bwd) == nullptr; }
-int tc_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s) { return run(p, g, s, false); }
-int tc_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s) { return run(p, g, s, true); }
+int tc_forward(const VilAttnParams* p, const Geo& g, cudaStream_t s, const int* image_hw) { return run(p, g, s, false, image_hw); }
+int tc_backward(const VilAttnParams* p, const Geo& g, cudaStream_t s, const int* image_hw) { return run(p, g, s, true, image_hw); }
 
 }  // namespace vil

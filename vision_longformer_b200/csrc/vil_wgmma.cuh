@@ -470,11 +470,13 @@ __device__ __forceinline__ void ring_wait(T* piece, T* fixed, int n0) {
 // ----------------------------------------------------------------------------------------------
 // held to 5 / 3 CTAs per SM (HD <= 32 / 64): left alone, ptxas spends registers on hoisting the column loads and drops one.
 // HD 128: 2, what the 2-stage ring fits (the O accumulator alone is 64 registers).  Split fp32 tiles: 4 / 3 / 2 (HD 16 /
-// 32 / 64); at 5 the HD 16 kernel, with its lo fragments, spills.
+// 32 / 64); at 5 the HD 16 kernel, with its lo fragments, spills.  DIL at HD 16: 4; at 5 it spills 24 bytes once the
+// sub-grid comes from a per-image size read from memory, which ptxas cannot rematerialise from the kernel parameters.
 template <typename T, int HD, typename TO, bool DROP = false, bool DIL = false>
-__global__ void __launch_bounds__(kThreads, kSplit<T> ? (HD <= 16 ? 4 : HD <= 32 ? 3 : 2) : HD <= 32 ? 5 : HD <= 64 ? 3 : 2)
+__global__ void __launch_bounds__(kThreads, kSplit<T> ? (HD <= 16 ? 4 : HD <= 32 ? 3 : 2)
+                                                      : HD <= 16 && DIL ? 4 : HD <= 32 ? 5 : HD <= 64 ? 3 : 2)
 wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const float* __restrict__ table,
-             const float* __restrict__ g2l) {
+             const float* __restrict__ g2l, const int* __restrict__ image_hw) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
   using W64 = sm90::Wg<Op<T>, 64>;
   using WHD = sm90::Wg<Op<T>, HD>;
@@ -492,7 +494,7 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
   const int tid = threadIdx.x, slot = tid >> 1, half = tid & 1;
   const int w = geo.w, D = geo.D;
   for (int i = tid; i < tabn; i += kThreads) tab[i] = table[(long long)i * geo.H + h];
-  const auto sg = sub_grid<DIL>(geo, R, C);
+  const auto sg = sub_grid<DIL>(geo, R, C, image_hw, b);
   if (off_sub_grid<DIL>(sg, R, C)) return;
   {
     const int l = cid.piece * 64 + slot;
@@ -591,11 +593,18 @@ wg_fwd_local(Geo geo, T4 q, T4 k, T4 v, T4 o, float* __restrict__ lse, const flo
 // TAB (the call has the bias table): the CTA is slice cid.b of the images and runs images cid.b, cid.b + nslice, ...;
 // after each chunk piece's dQ product its dS tile is added, in a fixed order, to the CTA's row of table partials tpart
 // (vil_common.cuh: table_grad_piece).  Without TAB, one image per CTA and none of that code.
-// HD 128 is held to 2 CTAs per SM, what the 2-stage ring fits; below it ptxas is left alone.
+// HD 128 is held to 2 CTAs per SM, what the 2-stage ring fits; below it ptxas is left alone, except for DIL at HD <= 32:
+// its sub-grid, read from memory for per-image sizes, cannot be rematerialised from the kernel parameters, and left alone
+// ptxas gives up a CTA per SM for it.  Held to the CTAs per SM the kernels had before per-image sizes, where that does
+// not spill: 3 with dropout, 4 without (split fp32 tiles; bf16 / fp16 at HD 32 with the table and HD 16 without).
+// bf16 / fp16 at HD 32 without the table stays at 3 (at 4 it spills 4 bytes), at HD 16 with the table at the 3 it had.
 template <typename T, int HD, typename TO, bool DROP = false, bool TAB = false, bool DIL = false>
-__global__ void __launch_bounds__(kThreads, kTileHD<T, HD> <= 64 ? 0 : 2)
+__global__ void __launch_bounds__(kThreads, kTileHD<T, HD> <= 64
+                                                ? (DIL && HD <= 32 ? (DROP ? 3 : kSplit<T> || HD == (TAB ? 32 : 16) ? 4 : 0) : 0)
+                                                : 2)
 wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ lse, const float* __restrict__ delta,
-          const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ tpart) {
+          const float* __restrict__ table, const float* __restrict__ g2l, float* __restrict__ tpart,
+          const int* __restrict__ image_hw) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
   using W64 = sm90::Wg<Op<T>, 64>;
   using WHD = sm90::Wg<Op<T>, HD>;
@@ -621,12 +630,17 @@ wg_bwd_dq(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dq, const float* __restrict__ ls
     acc = tpart + (long long)blockIdx.x * tabn;
     for (int i = tid; i < tabn; i += kThreads) acc[i] = 0.f;
   }
-  const auto sg = sub_grid<DIL>(geo, R, C);
-  if (off_sub_grid<DIL>(sg, R, C)) return;                       // after zeroing its row of table partials
+  auto sg = sub_grid<DIL>(geo, R, C, image_hw, cid.b);
+  // after zeroing its row of table partials; TAB: per image below, since the sub-grid depends on the image's size
+  if (!TAB && off_sub_grid<DIL>(sg, R, C)) return;
   const int nimg = TAB ? (geo.B - cid.b + geo.nslice - 1) / geo.nslice : 1;
   for (int it = 0; it < nimg; ++it) {
   const int b = cid.b + it * geo.nslice;
   const long long bh = (long long)b * geo.H + h;
+  if constexpr (TAB && DIL) {                                     // CTA-uniform: skip an image the chunk lies outside of
+    if (it > 0 && image_hw != nullptr) sg.fit(geo, image_hw, b);  // (dilated without sizes: the same sub-grid)
+    if (off_sub_grid<DIL>(sg, R, C)) continue;
+  }
   if (TAB && it > 0) __syncthreads();                             // the previous image is done with Qs, Gs, vl and the tile
   {
     const int l = cid.piece * 64 + slot;
@@ -855,7 +869,7 @@ __device__ __forceinline__ void dkv_probs(float (&s)[32], float (&dp)[32], const
 template <typename T, int HD, typename TO, bool DROP = false, bool DIL = false>
 __global__ void __launch_bounds__(kThreads, kSplit<T> ? (HD <= 16 ? 3 : 2) : HD > 64 ? 2 : (HD <= 32 ? 4 : 3) - (DROP ? 1 : 0))
 wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restrict__ lse, const float* __restrict__ delta,
-           const float* __restrict__ table) {
+           const float* __restrict__ table, const int* __restrict__ image_hw) {
   constexpr int HH = HD / 2, TILE = 64 * HD;
   using W64 = sm90::Wg<Op<T>, 64>;
   using WHD = sm90::Wg<Op<T>, HD>;
@@ -878,7 +892,7 @@ wg_bwd_dkv(Geo geo, T4 q, T4 k, T4 v, T4 d_o, T4 dk, T4 dv, const float* __restr
   const int w = geo.w, D = geo.D;
   const long long bh = (long long)b * geo.H + h;
   for (int i = tid; i < tabn; i += kThreads) tab[i] = table[(long long)i * geo.H + h];
-  const auto sg = sub_grid<DIL>(geo, KR, KC);
+  const auto sg = sub_grid<DIL>(geo, KR, KC, image_hw, b);
   if (off_sub_grid<DIL>(sg, KR, KC)) return;
   {
     const int lk = cid.piece * 64 + slot;

@@ -23,6 +23,7 @@ slidingchunk_2d.py they call.
 from __future__ import annotations
 
 import ctypes
+import operator
 from typing import Optional
 
 import torch
@@ -85,6 +86,52 @@ def _base_params(q, k, nx, ny, w, nglo, exact, mode, scale, impl, skip_mask=0, f
     return p
 
 
+def image_sizes_host(image_sizes, B: int, nx: int, ny: int) -> Optional[torch.Tensor]:
+    """Validate per-image token grids on the host: `image_sizes` is a sequence of B (h, w) pairs or a CPU integer tensor
+    of shape (B, 2), with 1 <= h <= nx and 1 <= w <= ny.  Returns them as a CPU int32 (B, 2) tensor, or None when
+    `image_sizes` is None or every image fills the nx x ny grid (the unsized operator, bit for bit)."""
+    if image_sizes is None:
+        return None
+    if isinstance(image_sizes, torch.Tensor):
+        if image_sizes.device.type != "cpu":
+            raise TypeError(f"image_sizes is on {image_sizes.device}: pass host data (a sequence of (h, w) or a CPU tensor); "
+                            "the sizes are validated on the host, which a device tensor would need a synchronise for")
+        if image_sizes.is_floating_point() or image_sizes.is_complex() or image_sizes.dtype == torch.bool:
+            raise TypeError(f"image_sizes must hold integers (got {image_sizes.dtype})")
+        t = image_sizes.to(torch.int64)
+    else:
+        try:
+            t = torch.tensor([[operator.index(v) for v in hw] for hw in image_sizes], dtype=torch.int64)
+        except TypeError as e:
+            raise TypeError(f"image_sizes must be a sequence of (h, w) integer pairs: {e}") from None
+    if tuple(t.shape) != (B, 2):
+        raise ValueError(f"image_sizes must have shape ({B}, 2), one (h, w) per image (got {tuple(t.shape)})")
+    bad = (t[:, 0] < 1) | (t[:, 0] > nx) | (t[:, 1] < 1) | (t[:, 1] > ny)
+    if bool(bad.any()):
+        b = int(bad.nonzero()[0, 0])
+        raise ValueError(f"image_sizes[{b}] = ({int(t[b, 0])}, {int(t[b, 1])}) is outside [1, {nx}] x [1, {ny}]")
+    if bool((t[:, 0] == nx).all()) and bool((t[:, 1] == ny).all()):
+        return None
+    return t.to(torch.int32)
+
+
+def image_sizes_device(image_sizes, B: int, nx: int, ny: int, device) -> Optional[torch.Tensor]:
+    """`image_sizes_host`, uploaded to `device` without a host synchronise (pinned memory, non-blocking copy)."""
+    t = image_sizes_host(image_sizes, B, nx, ny)
+    if t is None:
+        return None
+    return t.pin_memory().to(device, non_blocking=True)
+
+
+def _call(fn_plain, fn_sized, p: VilAttnParams, image_hw: Optional[torch.Tensor], device):
+    """One library call on `device`'s current stream: the sized entry point when per-image grids are given."""
+    with torch.cuda.device(device):            # launch on the tensors' device and on ITS current stream
+        stream = ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        if image_hw is None:
+            return fn_plain(ctypes.byref(p), stream)
+        return fn_sized(ctypes.byref(p), ctypes.c_void_p(image_hw.data_ptr()), stream)
+
+
 def _split_flag(x: torch.Tensor, impl: str) -> int:
     """VIL_FLAG_F32_SPLIT for an fp32 call that may use the tensor cores: torch's fp32 matmul precision allows TF32 or
     split-bf16 products.  `fp32_precision` is read rather than get_float32_matmul_precision() or matmul.allow_tf32,
@@ -123,7 +170,7 @@ def _workspace(p: VilAttnParams, backward: bool, device) -> torch.Tensor:
 
 def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx, ny, w, exact=0, mode=0,
                               scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0,
-                              dilation=1):
+                              dilation=1, image_sizes=None, _image_hw=None):
     """q:(B,H,Nloc,D) k,v:(B,H,N,D) qg:(B,H,g,D) kg,vg:(B,H,N,D) views; o/og preallocated output views.
     `flags`: VIL_FLAG_* of include/vil_attn.h (F32_OUT = 1: o / og are fp32 tensors - the parity build; F32_SPLIT = 4:
     fp32 operands on the wgmma tensor cores as split bf16 products).
@@ -131,11 +178,14 @@ def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx
     backward must be given the same three values.
     `dilation` d > 1: dilated sliding-chunk attention (VIL_FLAG_DILATED, include/vil_attn.h): each local query attends
     within its residue sub-grid of image positions (a + d r', b + d c'); the backward must be given the same d.
+    `image_sizes`: per-image token grids of a padded batch, host data of B (h, w) (see `vil_attention`); the backward
+    must be given the same sizes.
     Returns (lse (B,H,Nloc) fp32, lse_g (B,H,g) fp32 or None)."""
     _require_cuda(q, "q")
     B, H, Nloc, D = q.shape
     g = k.shape[2] - Nloc
     assert Nloc == nx * ny, "Global dimension does not match!"           # longformer2d.py:111
+    hw = _image_hw if _image_hw is not None else image_sizes_device(image_sizes, B, nx, ny, q.device)
     p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset,
                      dilation)
     lse = torch.empty(B, H, Nloc, dtype=torch.float32, device=q.device)
@@ -146,9 +196,8 @@ def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx
     p.lse, p.lse_g = _ptr(lse), _ptr(lse_g)
     p.bias_table, p.g2l, p.g2g = _ptr(table), _ptr(g2l), _ptr(g2g)
     ws = _workspace(p, False, q.device)
-    with torch.cuda.device(q.device):          # launch on the tensors' device and on ITS current stream
-        rc = _lib.load().vil_attn_fwd_sm100(ctypes.byref(p), ctypes.c_void_p(torch.cuda.current_stream(q.device).cuda_stream))
-    _lib.raise_for(rc)
+    lib = _lib.load()
+    _lib.raise_for(_call(lib.vil_attn_fwd_sm100, lib.vil_attn_fwd_sized_sm100, p, hw, q.device))
     del ws
     return lse, lse_g
 
@@ -156,10 +205,11 @@ def vil_attention_raw_forward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, *, nx
 def vil_attention_raw_backward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, lse, lse_g, d_o, d_og,
                                dq, dk, dv, dqg, dkg, dvg, d_table, d_g2l, d_g2g, *, nx, ny, w, exact=0, mode=0,
                                scale=1.0, impl="auto", skip_mask=0, flags=0, dropout_p=0.0, dropout_seed=0, dropout_offset=0,
-                               dilation=1):
+                               dilation=1, image_sizes=None, _image_hw=None):
     _require_cuda(q, "q")
     Nloc = q.shape[2]
     g = k.shape[2] - Nloc
+    hw = _image_hw if _image_hw is not None else image_sizes_device(image_sizes, q.shape[0], nx, ny, q.device)
     p = _base_params(q, k, nx, ny, w, g, exact, mode, scale, impl, skip_mask, flags, dropout_p, dropout_seed, dropout_offset,
                      dilation)
     p.q, p.k, p.v, p.o = _t4(q), _t4(k), _t4(v), _t4(o)
@@ -171,9 +221,8 @@ def vil_attention_raw_backward(q, k, v, qg, kg, vg, table, g2l, g2g, o, og, lse,
     p.bias_table, p.g2l, p.g2g = _ptr(table), _ptr(g2l), _ptr(g2g)
     p.d_bias_table, p.d_g2l, p.d_g2g = _ptr(d_table), _ptr(d_g2l), _ptr(d_g2g)
     ws = _workspace(p, True, q.device)
-    with torch.cuda.device(q.device):
-        rc = _lib.load().vil_attn_bwd_sm100(ctypes.byref(p), ctypes.c_void_p(torch.cuda.current_stream(q.device).cuda_stream))
-    _lib.raise_for(rc)
+    lib = _lib.load()
+    _lib.raise_for(_call(lib.vil_attn_bwd_sm100, lib.vil_attn_bwd_sized_sm100, p, hw, q.device))
     del ws
 
 
@@ -190,7 +239,8 @@ class _VilAttention(torch.autograd.Function):
     # `vil_attention` (not via cast_inputs, which would also round the fp32 bias tables to bf16).
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda")
-    def forward(ctx, q_all, kv, qg_all, kvg, table, g2l, g2g, H, nx, ny, w, nglo, exact, mode, scale, impl, dropout_p, dilation):
+    def forward(ctx, q_all, kv, qg_all, kvg, table, g2l, g2g, H, nx, ny, w, nglo, exact, mode, scale, impl, dropout_p, dilation,
+                image_sizes):
         _require_cuda(q_all, "q")
         B = q_all.shape[0]
         C = q_all.shape[2]
@@ -218,14 +268,16 @@ class _VilAttention(torch.autograd.Function):
         out = torch.empty(B, N, C, dtype=q_all.dtype, device=q_all.device)
         o = _heads(out, H)[:, :, g:]
         og = _heads(out, H)[:, :, :g] if g > 0 else None
+        hw = image_sizes_device(image_sizes, B, nx, ny, q_all.device)   # kept on the device for the backward
         seed, offset = _dropout_state(q_all.device, dropout_p)
         flags = _split_flag(q_all, impl)
         lse, lse_g = vil_attention_raw_forward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, nx=nx, ny=ny, w=w,
                                                exact=exact, mode=mode, scale=scale, impl=impl, flags=flags,
                                                dropout_p=dropout_p, dropout_seed=seed, dropout_offset=offset,
-                                               dilation=dilation)
+                                               dilation=dilation, _image_hw=hw)
         ctx.save_for_backward(q_all, kv, qg_all, kvg, table, g2l, g2g, out, lse, lse_g)
         ctx.cfg = (H, nx, ny, w, g, exact, mode, scale, impl, shared, flags, dilation)
+        ctx.hw = hw
         ctx.drop = (dropout_p, seed, offset)
         return out
 
@@ -266,15 +318,15 @@ class _VilAttention(torch.autograd.Function):
         vil_attention_raw_backward(q, k, v, qg, kg, vg, tab32, g2l32, g2g32, o, og, lse, lse_g, d_o, d_og,
                                    dq, dk, dv, dqg, dkg, dvg, d_tab, d_g2l, d_g2g, nx=nx, ny=ny, w=w, exact=exact,
                                    mode=mode, scale=scale, impl=impl, flags=flags, dropout_p=dropout_p,
-                                   dropout_seed=seed, dropout_offset=offset, dilation=dilation)
+                                   dropout_seed=seed, dropout_offset=offset, dilation=dilation, _image_hw=ctx.hw)
         cast = lambda d, ref: None if d is None else d.to(ref.dtype)
         return (dq_all, dkv, dqg_all, dkvg, cast(d_tab, table) if table is not None else None,
                 cast(d_g2l, g2l) if g2l is not None else None, cast(d_g2g, g2g) if g2g is not None else None,
-                None, None, None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None, None, None, None)
 
 
 def vil_attention(q_all, kv, qg_all=None, kvg=None, table=None, g2l=None, g2g=None, *, num_heads, nx, ny, w,
-                  nglo, exact=0, mode=0, scale=1.0, impl="auto", dropout_p=0.0, dilation=1):
+                  nglo, exact=0, mode=0, scale=1.0, impl="auto", dropout_p=0.0, dilation=1, image_sizes=None):
     """Fused local+global Vision-Longformer attention.
 
     shared weights (sharew):   q_all (B, nglo+nx*ny, C) = query(x);          kv (B, N, 2C) = kv(x)
@@ -293,13 +345,21 @@ def vil_attention(q_all, kv, qg_all=None, kvg=None, table=None, g2l=None, g2g=No
     columns congruent mod d); each local query attends to the global tokens and, with the same w / exact / mode / bias
     table, to the keys of its own sub-grid, so its window reaches w * d image positions.  Global queries are unchanged.
     d = 1 is the undilated operator, bit for bit.
+
+    `image_sizes`: per-image token grids of a padded batch (detection batches of images of different sizes).  Host data:
+    a sequence of B (h, w) pairs or a CPU integer tensor of shape (B, 2), 1 <= h <= nx, 1 <= w <= ny; image b's real
+    tokens are its top-left h x w of the nx x ny grid, in the padded layout.  Each real token gets exactly what the call
+    on image b alone, cropped to h x w, gives it (local and global queries, all gradients); the output rows of the
+    off-image local tokens are zeros and their gradients are zeros, and the contents of q / kv at those tokens never
+    reach any output.  Validated on the host (ValueError / TypeError) and uploaded without a host synchronise; with every
+    image at (nx, ny) this is the call without sizes.  Composes with dilation (the crop's residue sub-grids) and dropout.
     """
     if q_all.is_cuda and torch.is_autocast_enabled("cuda"):
         dt = torch.get_autocast_dtype("cuda")
         cast = lambda t: t if (t is None or t.dtype == dt) else t.to(dt)
         q_all, kv, qg_all, kvg = cast(q_all), cast(kv), cast(qg_all), cast(kvg)
     return _VilAttention.apply(q_all, kv, qg_all, kvg, table, g2l, g2g, num_heads, nx, ny, w, nglo, exact, mode,
-                               float(scale), impl, float(dropout_p), int(dilation))
+                               float(scale), impl, float(dropout_p), int(dilation), image_sizes)
 
 
 class _VilAttentionPacked(torch.autograd.Function):
